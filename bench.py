@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — molecules/s for 1000-step GCDM sampling with the B200-native GCPNet denoiser.
+"""bench.py — molecules/s for 1000-step GCDM sampling with the H100-native GCPNet denoiser.
 
 Contract (see DESIGN.md §Measurement):
   python bench.py --gpus N --steps K --warmup W            # our arm (torchrun for N > 1, one rank per GPU)
@@ -12,6 +12,8 @@ for N > 1 every GPU gets its own 128 molecules (weak scaling) and the final coor
 `--config geom_hist` is BASELINE config[3]: GEOM-Drugs, 512 molecules IN TOTAL with sizes drawn from the dataset's
 number-of-atoms histogram (seed 123), split over the ranks by bdiff.distributed.sample_sharded (LPT by n^2, strong
 scaling, one NCCL gather).  Rank 0 prints ONE JSON line.
+`--dump-outputs DIR` writes what the last timed step returned (the sampler's arrays) as DIR/<name>.npy; the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -45,10 +47,12 @@ def parse_args():
     ap.add_argument("--atoms", type=int, default=None, help="atoms per molecule (default 19 qm9 / 44 geom)")
     ap.add_argument("--timesteps", type=int, default=1000)
     ap.add_argument("--mode", default=os.environ.get("BDIFF_MODE", "tensor"), choices=["parity", "tensor"],
-                    help="tensor: tcgen05 GEMMs with split-bf16 (hi+lo, >=16-bit) operands and fp32 accumulation, <=1e-4 "
+                    help="tensor: wgmma GEMMs with split-bf16 (hi+lo, >=16-bit) operands and fp32 accumulation, <=1e-4 "
                          "from the reference per forward (default); parity: all-fp32 FFMA")
     ap.add_argument("--no-parity-leg", action="store_true", help="skip the extra fp32 parity-mode chain (tensor mode)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the arrays the last timed step returned as DIR/<name>.npy")
     ap.add_argument("--cpu-forwards", type=int, default=0,
                     help="denoiser forwards per CPU sample (bounded sample of the workload; default 8, geom_hist 2)")
     return ap.parse_args()
@@ -56,7 +60,7 @@ def parse_args():
 
 # ------------------------------------------------------------------------------------------------ clocks
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -237,20 +241,24 @@ def run_ours(args):
     E = int((sizes_mine.long() ** 2).sum())
     width = 3 + dcfg.num_atom_types + int(dcfg.include_charges)
     out_host = torch.empty((int(sizes_all.sum()) if strong else n_nodes, width), pin_memory=True)
-    flush_buf = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # > 126 MB L2
+    flush_buf = torch.empty(256 * 1024 * 1024 // 4, device=dev)      # > 50 MB L2
     finite_flag = torch.ones((), dtype=torch.bool, device=dev)
+    last_result = [None]
 
     def one_chain(nodes, ctx):
         """The product's public call for this workload; returns the step's result on the device."""
         nonlocal finite_flag
         if strong:
-            out, _ = sample_sharded(sampler, nodes, ctx, T)          # LPT shards, chain, ONE NCCL all_gather
+            result = sample_sharded(sampler, nodes, ctx, T)          # LPT shards, chain, ONE NCCL all_gather
+            out = result[0]
         else:
-            out, _, _ = sampler.sample(nodes, ctx, T)
+            result = sampler.sample(nodes, ctx, T)
+            out = result[0]
             if world > 1:
                 bufs = [torch.empty_like(out) for _ in range(world)]
                 dist.all_gather(bufs, out)                           # single NCCL gather of final coordinates
         finite_flag = finite_flag & torch.isfinite(out).all()
+        last_result[0] = result
         return out
 
     nodes_dev = num_nodes_host.to(dev)
@@ -306,6 +314,8 @@ def run_ours(args):
     secs = timed(chain_resident, args.steps)
     clk = clocks.stop() if rank == 0 else None
     launches = sampler_launches(sampler, net) - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_result[0], ("out", "batch_index", "node_mask") if not strong else ("out", "aux"))
     log(f"timed resident chains done: {secs:.2f} s for {args.steps}")
     secs_e2e = timed(chain_e2e, args.steps)
     log(f"timed e2e chains done: {secs_e2e:.2f} s")
@@ -358,25 +368,20 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json"))).get("tensor_fused" if fused else args.mode)
-    except Exception:
-        pass
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))    # H100 SXM data sheet
     achieved_gbs = bytes_alg / t_kernel / 1e9
     achieved_tf = launch_flops / t_kernel / 1e12
-    tensor_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))     # the kernel is timed inside a long step
-    kname = ("k_layers_tc (persistent tcgen05 kernel: the fused per-edge message MLP + segmented scatter-sum and the node "
+    tensor_peak = float(peaks.get("bf16_tflops_sustained", 989.0))     # H100 SXM data sheet, dense
+    kname = ("k_layers_tc (persistent wgmma kernel: the fused per-edge message MLP + segmented scatter-sum and the node "
              "update of all %d layers, tiles scheduled by dependency flags; split-bf16 operands: 3 MMAs per algorithmic "
              "product)" % L if fused
              else "k_edge_message (fp32 fused per-edge GCP message MLP + segmented scatter-sum)")
     common = {
-        "kernel": kname, "traffic": traffic, "algorithmic_bytes_per_launch": bytes_alg,
+        "kernel": kname, "algorithmic_bytes_per_launch": bytes_alg,
         "algorithmic_flops_per_launch": launch_flops, "kernel_ms": t_kernel * 1000,
         "hbm_achieved_gbs": achieved_gbs, "hbm_peak_gbs": hbm_peak, "hbm_frac": achieved_gbs / hbm_peak,
         "algorithmic_tflops": achieved_tf,
-        "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)",
+        "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (dense, 700 W card)",
         "note": "the fused pass is compute-bound by construction (~1.3 kFLOP/B, SURVEY.md fact 3); the HBM figure "
                 "(BASELINE.json's metric) is carried as hbm_* next to the binding roof.  `achieved` counts ALGORITHMIC "
                 "FLOPs of the reference's un-factored fp32 math; the tensor pipe executes 3 bf16 MMAs per product to reach "
@@ -437,7 +442,7 @@ def run_ours(args):
                            "kind": "port", "forwards_sampled": nf,
                            "max_abs_diff_vs_ours": float((ours - ref_out).abs().max().item()),
                            "note": "oracle port of the reference's PyG/torch_scatter algorithm run as un-fused PyTorch CUDA ops "
-                                   "on the same B200 and batch (edge index precomputed); denoiser forwards only, scaled to "
+                                   "on the same GPU and batch (edge index precomputed); denoiser forwards only, scaled to "
                                    "the T+1 forwards of a sample"}
             log(f"un-fused GPU port: {ms_fwd:.1f} ms/forward")
         except Exception as ex:      # a baseline leg must never take the measurement down
@@ -454,11 +459,10 @@ def run_ours(args):
                    "config_name": args.config, "molecules_total": total_mols, "molecules_this_rank": len(mine),
                    "timesteps": T, "denoiser_forwards_per_step": T + 1, "nodes_rank0": n_nodes, "edges_rank0": E,
                    "mode": args.mode,
-                   "precision": ("tensor mode: every GEMM on tcgen05 tensor cores with split-bf16 operands (activations and "
-                                 "weights each hi+lo, >=16 significant bits; A_hi.W_hi + A_lo.W_hi + A_hi.W_lo), fp32 "
-                                 "accumulation in TMEM, fp32 state, ex2/rcp activations; per-forward error vs the "
-                                 "reference's fp32 path <= 1e-4*max(1,|out|) (measured 4e-6..3.5e-5 relative on the six "
-                                 "reference fixtures, tests/test_gpu_tc.py), bit-identical reruns")
+                   "precision": ("tensor mode: every GEMM on the tensor cores (wgmma) with split-bf16 operands (activations "
+                                 "and weights each hi+lo, >=16 significant bits; A_hi.W_hi + A_lo.W_hi + A_hi.W_lo), fp32 "
+                                 "accumulation, fp32 state, ex2/rcp activations; per-forward error vs the reference's fp32 "
+                                 "path <= 1e-4*max(1,|out|) (tests/test_gpu_tc.py), bit-identical reruns")
                                 if args.mode == "tensor" else "parity mode: all fp32 FFMA, 1e-6 from the reference",
                    "weights": "random init of the named architecture (seed 7)",
                    "l2": "flushed between timed chains (256 MiB write); inside a chain the working set is "
@@ -472,6 +476,7 @@ def run_ours(args):
         "gpu_launches": int(launches) * world,
         "chains_finite": True, "nan_guard_hits": int(nan_hits.item()),
         "clocks": clk,
+        "gpu": gpu_info(local),
         "roofline": roofline,
     }
     if strong:
@@ -629,7 +634,7 @@ def run_train(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    tensor_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    tensor_peak = float(peaks.get("bf16_tflops_sustained", 989.0))
     mols = B * world * args.steps
     line = {
         "metric": "molecules/sec (GEOM-Drugs training step: forward + backward + gradient all-reduce + optimizer)",
@@ -648,13 +653,13 @@ def run_train(args):
                 "h2d_bytes_per_step": int(sum(v.numel() * v.element_size() for v in batches[0])), "d2h_bytes_per_step": 4},
         "gpu_launches": int(launches) * world,
         "library_calls": "GEMMs of the training pass are cuBLAS SGEMM calls (not counted in gpu_launches)",
-        "losses_finite": True, "clocks": clk, "phase_ms_batch0": phases,
+        "losses_finite": True, "clocks": clk, "gpu": gpu_info(local), "phase_ms_batch0": phases,
         "roofline": {"bound": "tensor", "achieved": flops / t_fb / 1e12, "peak": tensor_peak, "unit": "TFLOP/s",
                      "frac": flops / t_fb / 1e12 / tensor_peak, "traffic": None,
                      "kernel": "forward + backward of the training pass (cuBLAS SGEMMs + element kernels), batch 0",
                      "algorithmic_flops": flops, "ms": 1000 * t_fb,
                      "note": "fp32 SGEMM does not run on the tensor pipe: against the bf16 tensor peak this fraction is small "
-                             "by construction; it is reported so that the gap to a tcgen05 training pass is visible"},
+                             "by construction; it is reported so that the gap to a tensor-core training pass is visible"},
     }
     if world == 1 and not args.no_cpu_baseline:
         # the same objective on the host: autograd through the oracle port, first `cpu_mols` molecules of batch 0
@@ -675,6 +680,37 @@ def run_train(args):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def gpu_info(index):
+    """Name and power limit of the card: an absolute rate is only meaningful with them."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        info["power_limit_w"] = float(q.stdout.strip().splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.TimeoutExpired):
+        pass
+    return info
+
+
+def dump_outputs(directory, result, names, max_bytes=64 * 1024 * 1024):
+    """<directory>/<name>.npy per array: floats as float32, integers / masks as float64; over 64 MiB, a seeded row sample."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    arrays = {}
+    for name, t in zip(names, result):
+        if not isinstance(t, torch.Tensor):
+            continue
+        t = t.detach().cpu()
+        arrays[name] = t.float() if t.is_floating_point() else t.double()
+    total = sum(a.numel() * a.element_size() for a in arrays.values())
+    for name, a in arrays.items():
+        if total > max_bytes and a.dim() > 0 and a.shape[0] > 1:
+            keep = max(1, int(a.shape[0] * max_bytes / total))
+            rows = torch.randperm(a.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            a = a[rows]
+        np.save(os.path.join(directory, name + ".npy"), a.numpy())
 
 
 def sampler_launches(sampler, net):

@@ -1,4 +1,4 @@
-"""bdiff — B200-native GCPNet denoiser hot path of GCDM (bio-diffusion).
+"""bdiff — H100-native GCPNet denoiser hot path of GCDM (bio-diffusion).
 
 Public surface (mirrors the reference's seam, SURVEY.md §8b):
     GCPNetDynamicsB200   drop-in for src.models.components.gcpnet.GCPNetDynamics

@@ -1,4 +1,4 @@
-"""ctypes binding of libbdiff_sm100.so (the C ABI in include/bdiff.h).
+"""ctypes binding of libbdiff_sm90.so (the C ABI in include/bdiff.h).
 
 There is NO fallback: if the shared library is missing or cannot be loaded this module raises, and every
 product entry point that needs the GPU raises with it.
@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libbdiff_sm100.so")
+LIB_PATH = os.path.join(_HERE, "libbdiff_sm90.so")
 
 MODE_PARITY_FP32 = 0
 MODE_TENSOR = 1
@@ -35,7 +35,6 @@ PROTOTYPES = {
     "bdiff_weights_missing": (C.c_int32, [C.c_void_p]),
     "bdiff_prepare": (C.c_int32, [C.c_void_p, C.c_void_p]),
     "bdiff_selftest_split": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "bdiff_selftest_pair": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bdiff_plan_topology": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
                                         C.POINTER(C.c_int64)]),
     "bdiff_edge_index": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -92,7 +91,7 @@ def load():
         fn.restype = res
         fn.argtypes = args
     if lib.bdiff_abi_version() != 1:
-        raise BdiffError("libbdiff_sm100.so ABI version mismatch")
+        raise BdiffError("libbdiff_sm90.so ABI version mismatch")
     _lib = lib
     return lib
 

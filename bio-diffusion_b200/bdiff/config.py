@@ -1,7 +1,7 @@
 """Denoiser dimensions, derived from the reference's five Hydra config groups.
 
 Mirrors what GCPNetDynamics.__init__ reads (reference src/models/components/gcpnet.py:933-1039) and rejects
-loudly every option the B200 kernels do not implement (they implement exactly the shipped configs:
+loudly every option the CUDA kernels do not implement (they implement exactly the shipped configs:
 configs/model/{model_cfg,module_cfg,layer_cfg,diffusion_cfg}/*.yaml).
 """
 from __future__ import annotations

@@ -5,7 +5,7 @@ with strict=True, state-dict prefix `ddpm.dynamics_network.`), same call contrac
 
     forward(batch, xh[N,3+F], t[N,1], **kwargs) -> (batch, net_out[N,3+F])
 
-but every arithmetic step runs in libbdiff_sm100.so (hand-written sm_100a kernels).  To plug it into the
+but every arithmetic step runs in libbdiff_sm90.so (hand-written sm_90a kernels).  To plug it into the
 reference, add it to the `dynamics_networks` dict of src/models/qm9_mol_gen_ddpm.py:101-105 (INTEGRATION.md).
 There is no CPU / PyTorch fallback: tensors must live on a CUDA device and the library must be built.
 

@@ -1,9 +1,9 @@
-"""GCDMEvalNLL / GCDMTrainLoss — the GCDM objective with the B200 denoiser (forward only).
+"""GCDMEvalNLL / GCDMTrainLoss — the GCDM objective with the CUDA denoiser (forward only).
 
 Replaces EquivariantVariationalDiffusion.forward in eval mode (reference
 src/models/components/variational_diffusion.py:955-1160 with :501-556, :598-699, :702-732, :910-931) and the
 evaluation branch of the Lightning module's assembly (src/models/qm9_mol_gen_ddpm.py:184-262): two denoiser calls
-(t ~ U{1..T} and t = 0) through libbdiff_sm100, the scalar bookkeeping in torch on the same device.
+(t ~ U{1..T} and t = 0) through libbdiff_sm90, the scalar bookkeeping in torch on the same device.
 `GCDMTrainLoss` is the training-mode L2 objective of the same function (one denoiser call, t ~ U{0..T}, L0 selected
 by the t == 0 mask; :979-980,985,1054-1055,1068-1069,1083-1103 and qm9_mol_gen_ddpm.py:232-245).  Called with autograd
 enabled and trainable parameters it runs the library's training pass, so `loss.mean().backward()` fills `p.grad` of

@@ -1,4 +1,4 @@
-"""Optimiser side of a GCDM training step on the B200 library: adaptive gradient-norm clipping, AdamW(amsgrad) and the
+"""Optimiser side of a GCDM training step on the CUDA library: adaptive gradient-norm clipping, AdamW(amsgrad) and the
 EMA of the weights as three multi-tensor kernels (`bdiff_optimizer_step`, csrc/bdiff_optim.cu) — mirrors what the
 reference does with `configure_gradient_clipping` (qm9_mol_gen_ddpm.py:1267-1304), `torch.optim.AdamW`
 (configs/model/*_mol_gen_ddpm.yaml:3-8) and the `EMA` callback (src/utils/__init__.py:71-160) every step.

@@ -1,4 +1,4 @@
-"""GCDMSampler — the T-step ancestral sampler of GCDM with the B200 denoiser in its inner loop.
+"""GCDMSampler — the T-step ancestral sampler of GCDM with the CUDA denoiser in its inner loop.
 
 Replaces the inner loop of EquivariantVariationalDiffusion.mol_gen_sample / sample_p_zs_given_zt /
 sample_p_xh_given_z0 (reference src/models/components/variational_diffusion.py:1280-1412, 1204-1278, 840-907):

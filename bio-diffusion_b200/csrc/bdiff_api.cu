@@ -173,6 +173,7 @@ cudaError_t ensure_work(bdiff_handle* h) {
                o_PJ = take(Np * kPStride), o_agg = take(Np * kMsg), o_hp = take(Np * 32),
                o_e = take(Ep * d.Ed), o_xie = take(Ep * d.Xd * 3), o_fr = take(Ep * 9), o_pjt = take(Np * 256),
                o_mid = take(h->cfg.mode == BDIFF_MODE_TENSOR ? (Ep / 128) * kMsg : 0),
+               o_acc = take(h->cfg.mode == BDIFF_MODE_TENSOR ? (size_t)h->num_sms * TM_COLS * 128 : 0),
                o_flag = take(64);
   cudaError_t e = h->work_buf.ensure(off * sizeof(float));
   if (e != cudaSuccess) return e;
@@ -183,6 +184,7 @@ cudaError_t ensure_work(bdiff_handle* h) {
   w.e = b + o_e; w.xi = b + o_xie; w.frames = b + o_fr;
   w.PJT = h->cfg.mode == BDIFF_MODE_TENSOR ? b + o_pjt : nullptr;
   w.mid = h->cfg.mode == BDIFF_MODE_TENSOR ? b + o_mid : nullptr;
+  w.acc = h->cfg.mode == BDIFF_MODE_TENSOR ? b + o_acc : nullptr;
   w.npad = (int)Np;
   w.nan_flag = reinterpret_cast<int*>(b + o_flag);
   w.dbg = nullptr;
@@ -215,15 +217,15 @@ int32_t bdiff_create(const bdiff_config* cfg, bdiff_handle** out) {
   if (cfg->mode != BDIFF_MODE_PARITY_FP32 && cfg->mode != BDIFF_MODE_TENSOR) { g_create_error = "unknown mode"; return BDIFF_EINVAL; }
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) {
-    g_create_error = "no CUDA device: libbdiff_sm100 has no CPU fallback";
+    g_create_error = "no CUDA device: libbdiff_sm90 has no CPU fallback";
     return BDIFF_ECUDA;
   }
   cudaDeviceProp prop{};
   int dev = 0;
   cudaGetDevice(&dev);
   cudaGetDeviceProperties(&prop, dev);
-  if (prop.major != 10) {
-    g_create_error = "libbdiff_sm100 is built for sm_100a (B200) only; found compute capability " +
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "libbdiff_sm90 is built for sm_90a (H100) only; found compute capability " +
                      std::to_string(prop.major) + "." + std::to_string(prop.minor);
     return BDIFF_ECUDA;
   }
@@ -391,18 +393,6 @@ int32_t bdiff_selftest_split(void* stream, int32_t variant, const float* A, cons
   return e == cudaSuccess ? BDIFF_OK : BDIFF_ECUDA;
 }
 
-int32_t bdiff_selftest_pair(void* stream, const float* A, const float* W, float* C) {
-  if (!A || !W || !C) return BDIFF_EINVAL;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (selftest_pair_configure() != cudaSuccess) return BDIFF_ECUDA;
-  void* img = nullptr;
-  if (cudaMalloc(&img, selftest_pair_img_bytes()) != cudaSuccess) return BDIFF_ENOMEM;
-  launch_umma_selftest_pair(st, A, W, static_cast<unsigned char*>(img), C);
-  cudaError_t e = cudaStreamSynchronize(st);
-  cudaFree(img);
-  return e == cudaSuccess ? BDIFF_OK : BDIFF_ECUDA;
-}
-
 int32_t bdiff_weights_missing(const bdiff_handle* h) {
   if (!h) return BDIFF_EINVAL;
   int n = 0;
@@ -535,9 +525,10 @@ int32_t bdiff_plan_topology(bdiff_handle* h, void* stream, int32_t num_mols, int
   h->sched.TE = (int)ntile128;
   h->sched.TN = ntile32;
   {
-    // Claim order of the layer megakernel, in PAIR items: a CTA pair works on tiles (2j, 2j+1) of one kind and layer (the
-    // second tile of the last pair is a ghost when the count is odd).  Virtual time of edge pair (l, j) = l*PE + j; node pair
-    // (l, v) follows the last edge pair it reads by `lag` claims (about one wave: by then that pair has normally finished).
+    // Claim order of the layer megakernel, in PAIR items: item j holds tiles (2j, 2j+1) of one kind and layer, claimed one
+    // tile at a time (the second tile of the last pair is skipped when the count is odd).  Virtual time of edge pair (l, j) =
+    // l*PE + j; node pair (l, v) follows the last edge pair it reads by `lag` items (about one wave of num_sms tile claims:
+    // by then that pair has normally finished).
     // Every dependency must precede its consumer in the list (deadlock freedom), which bounds the lag: edge pair (l+1, j)
     // reads node pairs <= ndep(j), whose time is l*PE + edep(ndep) + lag  <  (l+1)*PE + j.
     const int L = h->d.L, TE = (int)ntile128, TN = ntile32;

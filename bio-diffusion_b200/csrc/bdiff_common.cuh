@@ -1,4 +1,4 @@
-// bdiff_common.cuh — shared definitions for libbdiff_sm100.so (sm_100a only).
+// bdiff_common.cuh — shared definitions for libbdiff_sm90.so (sm_90a only).
 //
 // Layout conventions (all fp32 unless noted):
 //   node tensors  h [N,256], chi [N,32*3] (channel-major, xyz-minor == ScalarVector.flatten order,
@@ -20,6 +20,7 @@ constexpr int kHidM = 8;      // hidden vector dim of G1..G3 / POS: 32 / bottlen
 constexpr int kHidFF = 16;    // hidden vector dim of the feed-forward GCP: 64 / 4
 constexpr int kKM = 280;      // padded fan-in of G1..G3 / POS scalar_out: 256 + 8 + 9 = 273 -> 280
 constexpr int kKFF = 540;     // padded fan-in of FF scalar_out.0: 512 + 16 + 9 = 537 -> 540
+constexpr int TM_COLS = 512;  // columns of the per-CTA accumulator scratch of the tensor path (bdiff_tc.cuh)
 constexpr int kPStride = 328; // per-node projection record: 256 + hid0*3 (<=60) + 9 -> 328
 constexpr int kKC = 16;       // K rows of a weight chunk staged in shared memory (16 x 256 x 4 B = 16 KiB)
 

@@ -1,5 +1,5 @@
 // bdiff_edge_tc.cuh — declarations of the tensor-core edge tile of the layer megakernel (bdiff_layers_tc.cu):
-// tile / TMEM constants, shared-memory layout, weight-slab stream, the per-thread vector-channel update.
+// tile / accumulator-scratch constants, shared-memory layout, weight-slab stream, the per-thread vector-channel update.
 #pragma once
 #include "bdiff_kernels.h"
 #include "bdiff_slab.cuh"
@@ -7,11 +7,11 @@
 namespace bdiff {
 
 constexpr int TMT = 128;                 // edges per tile
-// weight ring: TC_NSLOT slots of TC_SLOT bytes; a chunk is one slab plane (N rows x 32 B, N <= 320) or a group of
-// small planes, always a single contiguous TMA bulk copy
-constexpr int TC_SLOT = 2 * 160 * 32;    // 10 KiB: this CTA's half of the widest K step (hi plane + lo plane)
+// weight ring: TC_NSLOT slots of TC_SLOT bytes; a chunk is one K step of one N half of a weight plane (hi plane + lo
+// plane, N/2 rows x 32 B each) or a group of small K steps, always a single contiguous TMA bulk copy
+constexpr int TC_SLOT = 2 * 160 * 32;    // 10 KiB: one N half of the widest K step
 constexpr int TC_NSLOT = 5;
-// TMEM column map of an edge tile (512 columns allocated)
+// accumulator-scratch column map of an edge tile (512 columns)
 constexpr int TM_S = 0, TM_U0 = 256, TM_U1 = 288, TM_MV = 320, TM_VD0 = 416;
 constexpr int TM_EX = 416, TM_EX_STRIDE = 40;     // pair-exchange scratch (over VD0, which is dead by then): 2 x 40 columns
 
@@ -25,17 +25,16 @@ __host__ __device__ inline size_t tc_edge_stream_bytes(int Ed, int Xd) {
 
 // mbarriers / bookkeeping of the megakernel; first member (base class) of both tile tails
 struct TcBars {
-  uint64_t full[TC_NSLOT], empty[TC_NSLOT], pfull[TC_NSLOT], a_ready, d_full, wbar, u_free;
-  uint64_t item_full[2], item_empty[2], peer_empty[2], tile_done;
-  alignas(16) int item[2][4];   // work items {type, layer, tile of THIS CTA, -}; the leader writes the peer's copy (16-byte st.shared::cluster)
-  uint32_t tmem_ptr;
-  uint32_t pad_;
+  uint64_t full[TC_NSLOT], empty[TC_NSLOT], wbar;
+  uint64_t item_full[2], item_empty[2], tile_done;
+  alignas(16) int item[2][4];   // work items {type, layer, tile, -}
 };
 
 // Thread roles: warps 0-7 epilogue/compute — edge r of the tile is owned by the thread PAIR (r, r+128): "half" 0
 // works on accumulator columns [0,128) and vector channels [0,16), half 1 on columns [128,256) and channels
-// [16,32) (both warps of a pair address the same TMEM lanes: lane quarter = warp % 4); warp 8 = scheduler + TMA
-// producer (+ TMEM allocator), warp 9 = MMA issuer.
+// [16,32) (both warps of a pair address the same scratch rows: row quarter = warp % 4).  The two compute warpgroups
+// also issue the wgmmas (warpgroup g: tile rows [64 g, 64 g + 64)).  Warp 8 = scheduler + TMA producer, warp 9 =
+// completion-flag lane.
 constexpr int TC_EPI = 256;
 
 struct alignas(16) SmallW {   // fp32 copies of the thread-local (vector channel) weights, broadcast-read
@@ -59,7 +58,7 @@ struct EdgeTail : TcBars {
   uint32_t winfo[8];       // per window: start mask | end mask << 16
 };
 
-// Gate of the previous GCP from TMEM (U), vector-message update in TMEM scratch for this thread's 16 channels,
+// Gate of the previous GCP from the scratch (U), vector-message update in the scratch for this thread's 16 channels,
 // and this thread's partial vector_down / vector_down_frames sums of the NEXT GCP.
 // HP = hidden dim of the previous GCP; vdp = its vector_down output (full, [HP][3]).
 template <int HP, bool FIRST, bool LAST>
@@ -148,7 +147,7 @@ __device__ __forceinline__ void gate_update(uint32_t tl, int half, int ucol, con
   tmem_st_wait();
 }
 
-// The two threads of a pair (same TMEM lane) swap their 33 partial sums through TMEM scratch columns: no shared memory.
+// The two threads of a pair (same scratch row) swap their 33 partial sums through scratch columns.
 // Callers guarantee that nobody still reads the columns (VD0) being overwritten.
 __device__ __forceinline__ void pair_exchange33(uint32_t tl, int half, const float* __restrict__ mine, float* __restrict__ theirs) {
   float pad[40];

@@ -89,7 +89,7 @@ struct bdiff_handle {
   DevBuf tc_blob, tc_node_blob;
   size_t tc_layer_bytes = 0, tc_node_layer_bytes = 0;
   bool tc_dirty = true;
-  int num_sms = 148;
+  int num_sms = 132;
   cudaStream_t side = nullptr;          // fork/join stream: the edge embedding runs next to the node embedding
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 

@@ -29,6 +29,7 @@ struct Work {
   float* xi;       // [E,Xd*3]
   float* frames;   // [E,9]
   int* nan_flag;   // [0] NaN seen in this forward (gcpnet.py:1214-1216 guard), [1] forwards in which the guard fired (cumulative)
+  float* acc;      // tensor mode: [num_sms][512][128] accumulator scratch of the layer megakernel (one slice per CTA)
   long long* dbg;  // optional [CTA][64] clock64 stamps of the tensor-core kernels (BDIFF_TIMING=1), else nullptr
 };
 
@@ -74,20 +75,17 @@ struct LayerSched {
   const unsigned char* node_blob;
   size_t node_blob_stride;
   int L, TE, TN;                   // layers, 128-edge tiles, 32-node tiles
-  int nitems;                      // pair items in the work list: L * (ceil(TE/2) + ceil(TN/2))
+  int nitems;                      // items in the work list: L * (ceil(TE/2) + ceil(TN/2))
   int* sched;                      // [0] queue head, [1] unused, [2 + l*(TE+TN) + i] completion flags; zeroed per forward
   int* err;                        // sticky error word (dependency wait timed out); cleared when the plan is built / reported
   const int2* edge_dep;            // [TE] inclusive range of 32-node tiles whose previous-layer output an edge tile reads
   const int2* node_dep;            // [TN] inclusive range of edge tiles whose messages a node tile reads
-  const int* items;                // [nitems] work list in claim order: type<<30 | layer<<24 | PAIR index: a CTA pair works on tiles 2j, 2j+1 (see bdiff_plan_topology)
+  const int* items;                // [nitems] work list in claim order: type<<30 | layer<<24 | item j = tiles 2j, 2j+1, claimed one at a time (see bdiff_plan_topology)
 };
 cudaError_t tc_layers_configure();
 void launch_layers_tc(cudaStream_t st, const Plan& p, const Dims& d, const EmbedW& ew, const LayerSched& q,
                       const Work& w, int num_sms);
 cudaError_t selftest_configure();
-cudaError_t selftest_pair_configure();
-size_t selftest_pair_img_bytes();
-void launch_umma_selftest_pair(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C);
 size_t selftest_img_bytes();
 void launch_umma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
                                 int variant);

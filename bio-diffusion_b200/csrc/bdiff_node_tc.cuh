@@ -2,8 +2,8 @@
 //
 // Tile = 32 nodes.  The A operand uses the "R5" split-bf16 layout of bdiff_slab.cuh (each node row stored as
 // hi, lo, hi, lo, hi; two 128-row views and four products per K step), which leaves node l's complete accumulator row
-// in all four TMEM lane quarters: the 8 compute warps share the same 32 nodes, warp s owns accumulator columns
-// [32 s, 32 s + 32) (reachable in its own lane quarter) and 1/8 of the vector-channel work.
+// in all four row quarters of the accumulator scratch: the 8 compute warps share the same 32 nodes, warp s owns
+// accumulator columns [32 s, 32 s + 32) (read from its own row quarter) and 1/8 of the vector-channel work.
 #pragma once
 #include "bdiff_edge_tc.cuh"
 

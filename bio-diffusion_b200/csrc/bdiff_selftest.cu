@@ -1,11 +1,13 @@
-// bdiff_selftest.cu — hardware self test of the split-bf16 tcgen05 machinery used by the layer megakernel:
+// bdiff_selftest.cu — hardware self test of the split-bf16 wgmma machinery used by the layer megakernel:
 //   * A operand: 128B-swizzled K-major bf16 blocks, hi and lo blocks written by threads (x_store8_hl);
 //   * B operand: un-swizzled K=16 slabs [2 chunks][N rows][16 B] (hi plane, lo plane) fetched by TMA bulk copies
-//     and addressed with the SWIZZLE_NONE descriptor (umma_desc_k16);
-//   * three products per K step (A_hi.W_hi + A_lo.W_hi + A_hi.W_lo), N = 256 | 32 | 32 (the last one negated);
+//     and addressed with the SWIZZLE_NONE descriptor (gmma_desc_k16);
+//   * three products per K step (A_hi.W_hi + A_lo.W_hi + A_hi.W_lo), N = 128 | 128 | 32 | 32 (the last one negated),
+//     each of the two warpgroups on its 64 rows;
 //   * variant bit 1: the node-tile "R5" layout (32 distinct rows stored as hi, lo, hi, lo, hi in 160-row blocks;
-//     two row views 0 / +32 and four products leave the complete sum in every TMEM lane quarter);
-//   * a TMEM scratch round trip between the two threads that share a lane (the pair exchange of the edge tile).
+//     two row views 0 / +32 and four products leave the complete sum in every row quarter);
+//   * the accumulator scratch: fragment stores, and a round trip between the two threads that share a row (the pair
+//     exchange of the edge tile).
 // tests/test_gpu_tc.py compares C with an fp64 matmul at 3e-5 relative before the fused kernel is trusted.
 #include "bdiff_kernels.h"
 #include "bdiff_tc.cuh"
@@ -16,6 +18,7 @@ namespace bdiff {
 constexpr int ST_K = 128, ST_N = 320, ST_STEPS = ST_K / 16;
 constexpr int ST_SLAB = ST_N * 32;                       // bytes of one plane of one K step
 constexpr size_t ST_SMEM = 4 * (size_t)X_BLOCK + (size_t)ST_STEPS * 2 * ST_SLAB + 64 + 1024;
+constexpr size_t ST_IMG = (size_t)ST_STEPS * 2 * ST_SLAB;   // packed weights, followed by the accumulator scratch
 
 __global__ void k_selftest_pack_slabs(const float* __restrict__ W, unsigned char* __restrict__ img) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -24,27 +27,57 @@ __global__ void k_selftest_pack_slabs(const float* __restrict__ W, unsigned char
   slab_store(img + (size_t)(k >> 4) * 2 * ST_SLAB, ST_N, n, k & 15, W[idx]);
 }
 
+// columns [n0, n0 + N) of A . W^T (SA = -1: negated) for this warpgroup's 64 rows -> accumulator scratch
+template <int N, int SA>
+__device__ __forceinline__ void selftest_gemm(uint32_t xa, uint32_t wb, bool r5, int n0) {
+  float d[N / 2];
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+  wgmma_fence();
+  for (int ks = 0; ks < ST_STEPS; ++ks) {
+    const uint32_t bh = wb + (uint32_t)ks * 2 * ST_SLAB + n0 * 16, bl = bh + ST_SLAB;
+    const int j = ks >> 2, s = ks & 3;
+    uint64_t a0, a1;
+    if (!r5) {
+      a0 = gmma_desc_sw128(xa + j * X_BLOCK + s * 32);            // A_hi
+      a1 = gmma_desc_sw128(xa + (2 + j) * X_BLOCK + s * 32);      // A_lo
+    } else {
+      a0 = gmma_desc_sw128(xa + j * R5_BLOCK + s * 32);           // view 0:  hi lo hi lo
+      a1 = gmma_desc_sw128(xa + j * R5_BLOCK + 4096 + s * 32);    // view 32: lo hi lo hi
+    }
+    const uint64_t dh = gmma_desc_k16(bh, ST_N * 16, 128), dl = gmma_desc_k16(bl, ST_N * 16, 128);
+    // products: edge layout (A_hi,W_hi) (A_lo,W_hi) (A_hi,W_lo);  R5: (v0,W_hi) (v32,W_hi) (v0,W_lo) (v32,W_lo)
+    if (N == 128) {
+      wgmma_n128<SA>(d, a0, dh); wgmma_n128<SA>(d, a1, dh); wgmma_n128<SA>(d, a0, dl);
+      if (r5) wgmma_n128<SA>(d, a1, dl);
+    } else {
+      wgmma_n32<SA>(d, a0, dh); wgmma_n32<SA>(d, a1, dh); wgmma_n32<SA>(d, a0, dl);
+      if (r5) wgmma_n32<SA>(d, a1, dl);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  acc_fence<N / 2>(d);
+  acc_store<N>(d, n0, threadIdx.x >> 7);
+}
+
 __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __restrict__ A,
                                                                  const unsigned char* __restrict__ wimg,
-                                                                 float* __restrict__ C, int variant) {
+                                                                 float* __restrict__ scratch, float* __restrict__ C,
+                                                                 int variant) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   unsigned char* X = smem;                           // edge layout: hi blocks 0,1 | lo blocks 2,3;  R5 layout: 2 blocks x 20 KiB
   unsigned char* Wb = smem + 4 * X_BLOCK;
   uint64_t* bars = reinterpret_cast<uint64_t*>(Wb + (size_t)ST_STEPS * 2 * ST_SLAB);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
   const int tid = threadIdx.x, warp = tid >> 5;
-  const bool swap = variant & 1, r5 = variant & 2;
+  const bool r5 = variant & 2;
   if (tid == 0) {
     mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
     mbar_fence_init();
+    tm_base = scratch;
   }
-  if (warp == 8) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
   if (tid < 128) {
     if (!r5) {
       for (int k8 = 0; k8 < ST_K / 8; ++k8) {
@@ -68,121 +101,22 @@ __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __r
     for (int s = 0; s < ST_STEPS * 2; ++s) bulk_g2s(Wb + (size_t)s * ST_SLAB, wimg + (size_t)s * ST_SLAB, ST_SLAB, &bars[0]);
   }
   __syncthreads();
-  if (tid == 288 && variant >= 16) {
-    // ---- timing mode (tools/mma_timing.py): cycles of MMA streams of different shapes issued by one thread, A hi/lo blocks
-    // and the resident weight planes as operands (values irrelevant).  C[0] = cycles, C[1] = number of MMAs.
+  if (tid < 256) {
     mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    const uint32_t xa = smem_u32(X), wb0 = smem_u32(Wb);
-    const uint64_t adh = umma_desc_sw128(xa), adl = umma_desc_sw128(xa + 2 * X_BLOCK);
-    auto bdesc = [&](int ks, int pl, int row0) { return umma_desc_k16(wb0 + (uint32_t)((ks & 7) * 2 + pl) * ST_SLAB + row0 * 16, ST_N * 16, 128); };
-    auto adesc = [&](int ks, bool lo) { return (lo ? adl : adh) + (uint64_t)((((ks >> 2) & 1) * X_BLOCK + (ks & 3) * 32) >> 4); };
-    int n = 0;
-    const long long t0 = clock64();
-    if (variant >= 16 && variant <= 19) {
-      const int N = variant == 16 ? 256 : variant == 17 ? 32 : variant == 18 ? 64 : 160;
-      const uint32_t id = umma_idesc_bf16(N, false);
-      for (int ks = 0; ks < 32; ++ks)
-        for (int pr = 0; pr < 3; ++pr) { umma_bf16(tmem, adesc(ks, pr == 1), bdesc(ks, pr == 2, 0), id, true); ++n; }
-    } else if (variant == 20) {          // round-1/2a pattern: (256 | 32 | 32) x 3 products
-      const uint32_t i256 = umma_idesc_bf16(256, false), i32 = umma_idesc_bf16(32, false), i32n = umma_idesc_bf16(32, true);
-      for (int ks = 0; ks < 16; ++ks)
-        for (int pr = 0; pr < 3; ++pr) {
-          const uint64_t ad = adesc(ks, pr == 1);
-          umma_bf16(tmem, ad, bdesc(ks, pr == 2, 0), i256, true);
-          umma_bf16(tmem + 256, ad, bdesc(ks, pr == 2, 256), i32, true);
-          umma_bf16(tmem + 288, ad, bdesc(ks, pr == 2, 288), i32n, true);
-          n += 3;
-        }
-    } else if (variant == 21) {          // (256 | 64) x 3
-      const uint32_t i256 = umma_idesc_bf16(256, false), i64 = umma_idesc_bf16(64, false);
-      for (int ks = 0; ks < 16; ++ks)
-        for (int pr = 0; pr < 3; ++pr) {
-          const uint64_t ad = adesc(ks, pr == 1);
-          umma_bf16(tmem, ad, bdesc(ks, pr == 2, 0), i256, true);
-          umma_bf16(tmem + 256, ad, bdesc(ks, pr == 2, 256), i64, true);
-          n += 2;
-        }
-    } else if (variant == 22) {          // (160 | 160) x 3
-      const uint32_t i160 = umma_idesc_bf16(160, false);
-      for (int ks = 0; ks < 16; ++ks)
-        for (int pr = 0; pr < 3; ++pr) {
-          const uint64_t ad = adesc(ks, pr == 1);
-          umma_bf16(tmem, ad, bdesc(ks, pr == 2, 0), i160, true);
-          umma_bf16(tmem + 160, ad, bdesc(ks, pr == 2, 160), i160, true);
-          n += 2;
-        }
-    } else if (variant >= 24 && variant <= 26) {   // (160 | 160) x 3 with the megakernel's per-plane bookkeeping
-      // 24: per plane one (already satisfied) full-barrier wait + fence and one commit;  25: waits per plane, ONE commit per
-      // K step;  26: commits per plane, no waits
-      const uint32_t i160 = umma_idesc_bf16(160, false);
-      if (tid == 288) { mbar_init(&bars[2], 1); mbar_init(&bars[3], 1); mbar_fence_init(); }
-      for (int ks = 0; ks < 16; ++ks)
-        for (int pl = 0; pl < 2; ++pl) {
-          if (variant != 26) { mbar_wait(&bars[0], 0); tc_fence_after(); }
-          for (int pr = 0; pr < (pl == 0 ? 2 : 1); ++pr) {
-            const uint64_t ad = adesc(ks, pl == 0 && pr == 1);
-            umma_bf16(tmem, ad, bdesc(ks, pl, 0), i160, true);
-            umma_bf16(tmem + 160, ad, bdesc(ks, pl, 160), i160, true);
-            n += 2;
-          }
-          if (variant != 25 || pl == 1) umma_commit(&bars[2 + (pl & 1)]);
-        }
-    } else if (variant == 23) {          // 4 products of N=256 (node tile) x 16
-      const uint32_t i256 = umma_idesc_bf16(256, false);
-      for (int ks = 0; ks < 16; ++ks)
-        for (int pr = 0; pr < 4; ++pr) { umma_bf16(tmem, adesc(ks, pr & 1), bdesc(ks, pr >> 1, 0), i256, true); ++n; }
-    }
-    const long long t1 = clock64();
-    umma_commit(&bars[1]);
-    mbar_wait(&bars[1], 0);
-    const long long t2 = clock64();
-    C[0] = (float)(t2 - t0); C[1] = (float)n; C[2] = (float)(t1 - t0);
-  }
-  if (tid == 288 && variant < 16) {
-    mbar_wait(&bars[0], 0);
-    tc_fence_after();
-    const uint32_t i256 = umma_idesc_bf16(256, false), i32 = umma_idesc_bf16(32, false), i32n = umma_idesc_bf16(32, true);
-    const uint32_t lbo = swap ? 128u : (uint32_t)ST_N * 16u, sbo = swap ? (uint32_t)ST_N * 16u : 128u;
-    for (int ks = 0; ks < ST_STEPS; ++ks) {
-      const uint32_t bh = smem_u32(Wb) + (uint32_t)ks * 2 * ST_SLAB, bl = bh + ST_SLAB;
-      const int j = ks >> 2, s = ks & 3;
-      uint64_t a0, a1;
-      int na;
-      if (!r5) {
-        a0 = umma_desc_sw128(smem_u32(X) + j * X_BLOCK + s * 32);            // A_hi
-        a1 = umma_desc_sw128(smem_u32(X) + (2 + j) * X_BLOCK + s * 32);      // A_lo
-        na = 3;
-      } else {
-        a0 = umma_desc_sw128(smem_u32(X) + j * R5_BLOCK + s * 32);           // view 0:  hi lo hi lo
-        a1 = umma_desc_sw128(smem_u32(X) + j * R5_BLOCK + 4096 + s * 32);    // view 32: lo hi lo hi
-        na = 4;
-      }
-      for (int pr = 0; pr < na; ++pr) {
-        // products: edge layout (A_hi,W_hi) (A_lo,W_hi) (A_hi,W_lo);  R5: (v0,W_hi) (v32,W_hi) (v0,W_lo) (v32,W_lo)
-        const uint64_t ad = r5 ? ((pr & 1) ? a1 : a0) : (pr == 1 ? a1 : a0);
-        const uint32_t wb = r5 ? (pr >= 2 ? bl : bh) : (pr == 2 ? bl : bh);
-        const bool acc = (ks | pr) > 0;
-        umma_bf16(tmem + 0, ad, umma_desc_k16(wb, lbo, sbo), i256, acc);
-        umma_bf16(tmem + 256, ad, umma_desc_k16(wb + 256 * 16, lbo, sbo), i32, acc);
-        umma_bf16(tmem + 288, ad, umma_desc_k16(wb + 288 * 16, lbo, sbo), i32n, acc);
-      }
-    }
-    umma_commit(&bars[1]);
-  }
-  if (tid < 256 && variant < 16) {
-    mbar_wait(&bars[1], 0);
-    tc_fence_after();
+    const uint32_t xa = smem_u32(X) + (uint32_t)(tid >> 7) * 8192u, wb = smem_u32(Wb);
+    selftest_gemm<128, 1>(xa, wb, r5, 0);
+    selftest_gemm<128, 1>(xa, wb, r5, 128);
+    selftest_gemm<32, 1>(xa, wb, r5, 256);
+    selftest_gemm<32, -1>(xa, wb, r5, 288);
+    named_bar_sync(3, 256);
     const int half = tid >> 7, r = tid & 127;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    // pair exchange through TMEM scratch: each half writes 8 values into its own columns, reads the partner's
+    const uint32_t tl = (uint32_t)((warp & 3) * 32) << 16;
+    // pair exchange through the scratch: each half writes 8 values into its own columns, reads the partner's
     float mine[8], theirs[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) mine[i] = (float)(1000 * half + r * 8 + i);
     tmem_st8(tl + 320 + half * 8, mine);
-    tc_fence_before();
     named_bar_sync(3, 256);
-    tc_fence_after();
     tmem_ld8(tl + 320 + (half ^ 1) * 8, theirs);
     for (int c0 = half * 160; c0 < half * 160 + 160; c0 += 32) {
       float v[32];
@@ -192,120 +126,9 @@ __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __r
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) C[(size_t)r * 336 + 320 + half * 8 + i] = theirs[i];
-    tc_fence_before();
   }
-  __syncthreads();
-  if (warp == 8) tmem_dealloc(tmem, 512);
 }
 
-
-// -------------------------------------------------------------------------------------------- CTA-pair self test
-// C[256][320] = A[256][128] . W[320][128]^T with cta_group::2 MMAs: a cluster of two CTAs, each with its own 128 A rows
-// (hi / lo blocks) and its own TMEM, while every weight plane is split between the two shared memories: CTA c holds plane
-// rows [80 c, 80 c + 80) for the first N=160 MMA and [160 + 80 c, 240 + 80 c) for the second one (local rows 80..159).
-// The peer's TMA completion is relayed to the leader by a remote mbarrier arrive; the leader's commit is multicast to both
-// CTAs.  This is the machinery the next version of the layer megakernel needs to halve its shared-memory traffic.
-constexpr int SP_LOCAL = 160;                               // plane rows per CTA
-constexpr int SP_SLAB = SP_LOCAL * 32;                      // bytes of one local plane of one K step
-constexpr size_t SP_SMEM = 4 * (size_t)X_BLOCK + (size_t)ST_STEPS * 2 * SP_SLAB + 128 + 1024;
-
-__global__ void k_selftest_pack_pair(const float* __restrict__ W, unsigned char* __restrict__ img) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= ST_N * ST_K) return;
-  const int n = idx / ST_K, k = idx - n * ST_K;
-  const int mma = n / 160, within = n % 160, cta = within / 80, local = mma * 80 + within % 80;
-  // image = [cta][K step][hi plane | lo plane] with planes of SP_LOCAL rows
-  slab_store(img + ((size_t)cta * ST_STEPS + (k >> 4)) * 2 * SP_SLAB, SP_LOCAL, local, k & 15, W[idx]);
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(320, 1)
-    k_umma_selftest_pair(const float* __restrict__ A, const unsigned char* __restrict__ wimg, float* __restrict__ C) {
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* X = smem;
-  unsigned char* Wb = smem + 4 * X_BLOCK;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(Wb + (size_t)ST_STEPS * 2 * SP_SLAB);   // [0] full (local), [1] peer full (leader), [2] done
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t rank = cluster_ctarank();
-  if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&bars[2], 1);
-    mbar_fence_init();
-  }
-  cluster_sync_all();                                  // barriers of both CTAs initialised before any remote arrive
-  if (warp == 8) tmem_alloc2(tmem_ptr, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
-  if (tid < 128) {
-    for (int k8 = 0; k8 < ST_K / 8; ++k8) {
-      float v[8];
-#pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = A[((size_t)rank * 128 + tid) * ST_K + k8 * 8 + q];
-      x_store8_hl(X, 2, tid, k8 * 8, v);
-    }
-    fence_proxy_async();
-  }
-  if (tid == 256) {                                    // TMA lane: this CTA's half of every plane
-    mbar_expect_tx(&bars[0], ST_STEPS * 2 * SP_SLAB);
-    const unsigned char* src = wimg + (size_t)rank * ST_STEPS * 2 * SP_SLAB;
-    for (int s = 0; s < ST_STEPS * 2; ++s) bulk_g2s(Wb + (size_t)s * SP_SLAB, src + (size_t)s * SP_SLAB, SP_SLAB, &bars[0]);
-  }
-  __syncthreads();
-  cluster_sync_all();                                  // both A tiles written and visible to the async proxy of the pair
-  if (tid == 288) {
-    mbar_wait(&bars[0], 0);                            // my half has landed
-    if (rank == 1) {
-      mbar_arrive_remote(mapa_u32(&bars[1], 0));       // relay to the leader
-    } else {
-      mbar_wait(&bars[1], 0);                          // the peer's half has landed
-      tc_fence_after();
-      const uint32_t i160 = umma_idesc_bf16_m256(160);
-      for (int ks = 0; ks < ST_STEPS; ++ks) {
-        const uint32_t bh = smem_u32(Wb) + (uint32_t)ks * 2 * SP_SLAB, bl = bh + SP_SLAB;
-        const int j = ks >> 2, s = ks & 3;
-        const uint64_t ah = umma_desc_sw128(smem_u32(X) + j * X_BLOCK + s * 32);
-        const uint64_t al = umma_desc_sw128(smem_u32(X) + (2 + j) * X_BLOCK + s * 32);
-        for (int pr = 0; pr < 3; ++pr) {
-          const uint64_t ad = pr == 1 ? al : ah;
-          const uint32_t wb = pr == 2 ? bl : bh;
-          const bool acc = (ks | pr) > 0;
-          umma_bf16_pair(tmem + 0, ad, umma_desc_k16(wb, SP_LOCAL * 16, 128), i160, acc);
-          umma_bf16_pair(tmem + 160, ad, umma_desc_k16(wb + 80 * 16, SP_LOCAL * 16, 128), i160, acc);
-        }
-      }
-      umma_commit_pair(&bars[2]);
-    }
-  }
-  if (tid < 256) {
-    mbar_wait(&bars[2], 0);
-    tc_fence_after();
-    const int half = tid >> 7, r = tid & 127;
-    const uint32_t tl = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    for (int c0 = half * 160; c0 < half * 160 + 160; c0 += 32) {
-      float v[32];
-      tmem_ld32(tl + c0, v);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) C[((size_t)rank * 128 + r) * 320 + c0 + i] = v[i];
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  cluster_sync_all();                                  // nobody leaves while the pair's TMEM / barriers are in use
-  if (warp == 8) tmem_dealloc2(tmem, 512);
-}
-
-cudaError_t selftest_pair_configure() {
-  return cudaFuncSetAttribute(k_umma_selftest_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SP_SMEM);
-}
-void launch_umma_selftest_pair(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C) {
-  k_selftest_pack_pair<<<(ST_N * ST_K + 255) / 256, 256, 0, st>>>(W, img_scratch);
-  k_umma_selftest_pair<<<2, 320, SP_SMEM, st>>>(A, img_scratch, C);
-}
-size_t selftest_pair_img_bytes() { return (size_t)2 * ST_STEPS * 2 * SP_SLAB; }
 
 cudaError_t selftest_configure() {
   return cudaFuncSetAttribute(k_umma_selftest_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ST_SMEM);
@@ -314,9 +137,9 @@ cudaError_t selftest_configure() {
 void launch_umma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
                                 int variant) {
   k_selftest_pack_slabs<<<(ST_N * ST_K + 255) / 256, 256, 0, st>>>(W, img_scratch);
-  k_umma_selftest_split<<<1, 320, ST_SMEM, st>>>(A, img_scratch, C, variant);
+  k_umma_selftest_split<<<1, 320, ST_SMEM, st>>>(A, img_scratch, reinterpret_cast<float*>(img_scratch + ST_IMG), C, variant);
 }
 
-size_t selftest_img_bytes() { return (size_t)ST_STEPS * 2 * ST_SLAB; }
+size_t selftest_img_bytes() { return ST_IMG + (size_t)TM_COLS * 128 * sizeof(float); }
 
 }  // namespace bdiff

@@ -7,7 +7,7 @@
 //   node tile  : 5 blocks of [160 rows][64] ("R5"): node l of the 32-node tile is stored as hi in rows l, l+64, l+128
 //                and as lo in rows l+32, l+96.  The MMA reads the block through two 128-row views (row 0: hi lo hi lo,
 //                row 32: lo hi lo hi); view0.W_hi + view32.W_hi + view0.W_lo + view32.W_lo leaves the complete
-//                (hi+lo)(W_hi+W_lo) product in all four TMEM lane quarters, so the 8 compute warps keep sharing the 32
+//                (hi+lo)(W_hi+W_lo) product in all four row quarters of the accumulator, so the 8 compute warps keep sharing the 32
 //                nodes exactly as in the row-replicated bf16 kernel of round 1.
 // B operand (weights, packed once per weight update): "slabs" of one K=16 step:
 //                [hi plane | lo plane], plane = [2 K-chunks][N rows][16 bytes], un-swizzled (SWIZZLE_NONE, LBO = N*16,

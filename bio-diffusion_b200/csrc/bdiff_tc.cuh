@@ -1,11 +1,13 @@
-// bdiff_tc.cuh — tcgen05 / TMEM / UMMA-descriptor helpers for the tensor-core edge pass (sm_100a).
+// bdiff_tc.cuh — wgmma / shared-memory-descriptor helpers and the accumulator scratch of the tensor-core path (sm_90a).
 //
-// Conventions used by every UMMA operand in this library (bf16, K-major, 128-byte swizzle):
-//   an operand "K-block" is [rows][64 bf16] = rows x 128 B, 1024-byte aligned; element (r, k) lives at
+// Conventions used by every wgmma operand in this library (bf16, K-major):
+//   A: an operand "K-block" is [rows][64 bf16] = rows x 128 B, 1024-byte aligned, 128-byte swizzle; element (r, k) lives at
 //       r*128 + (((k >> 3) ^ (r & 7)) << 4) + (k & 7)*2            (the TMA SWIZZLE_128B pattern)
-//   the shared-memory descriptor points at the block (plus 32 B per K=16 step, plus r0*128 for a row offset
-//   that is a multiple of 8), SBO = 1024 B (8 rows), LBO unused, version 1, layout SWIZZLE_128B.
-//   Accumulators: M=128 rows -> TMEM lanes 0..127, N columns -> consecutive 32-bit TMEM columns.
+//     the descriptor points at the block (plus 32 B per K=16 step, plus r0*128 for a row offset that is a multiple of 8),
+//     SBO = 1024 B (8 rows), layout SWIZZLE_128B.  A warpgroup's M=64 rows start 64*128 = 8 KiB further on.
+//   B: un-swizzled K=16 slabs (see bdiff_slab.cuh), descriptor with explicit LBO / SBO.
+//   Accumulators: registers of the issuing warpgroup, stored at the end of a GEMM phase to a per-CTA scratch of 128 rows
+//   x 512 columns (column-major) that the epilogue threads read by row; scratch addresses are (row << 16) | column.
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -18,213 +20,148 @@ __device__ __forceinline__ uint32_t sw128_offset(int r, int k) {   // byte offse
   return (uint32_t)(r * 128 + ((((k >> 3) ^ (r & 7)) & 7) << 4) + (k & 7) * 2);
 }
 
-// 64-bit UMMA shared-memory descriptor for a K-major SWIZZLE_128B operand at byte address `saddr`.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// 64-bit wgmma shared-memory descriptor for a K-major SWIZZLE_128B operand at byte address `saddr`.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);          // start address  [0,14)
-  d |= (uint64_t)0 << 16;                          // leading byte offset [16,30): unused (one atom along K)
+  d |= (uint64_t)1 << 16;                          // leading byte offset [16,30): unused for a swizzled K-major operand
   d |= (uint64_t)((1024 >> 4) & 0x3FFF) << 32;     // stride byte offset  [32,46): 8 rows * 128 B
-  d |= (uint64_t)1 << 46;                          // descriptor version  [46,48) = 1 on sm_100
-  d |= (uint64_t)2 << 61;                          // layout type [61,64): SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                          // layout type [62,64): SWIZZLE_128B
   return d;
 }
 
-// 32-bit instruction descriptor, kind::f16: D=f32, A=B=bf16, both K-major, M=128, N given.
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int n, bool negate_a) {
-  uint32_t d = 0;
-  d |= 1u << 4;                    // c_format = F32
-  d |= 1u << 7;                    // a_format = BF16
-  d |= 1u << 10;                   // b_format = BF16
-  d |= (negate_a ? 1u : 0u) << 13; // a_negate
-  d |= (uint32_t)(n >> 3) << 17;   // n_dim
-  d |= (uint32_t)(128 >> 4) << 24; // m_dim
+// 64-bit wgmma descriptor for a K-major operand WITHOUT swizzle: core matrices of 8 rows x 16 bytes are contiguous
+// (128 B); consecutive 8-row groups are `sbo` bytes apart, the two 16-byte K chunks of one K=16 step `lbo` bytes apart.
+__device__ __forceinline__ uint64_t gmma_desc_k16(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
   return d;
 }
 
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          bool accumulate) {
+// D[64 x N] += (SA * A[64 x 16]) . B[N x 16]^T, bf16 operands from shared memory, fp32 accumulators in registers
+// (fragment of thread t of the warpgroup: see acc_store).  SA = -1 negates the product.
+template <int SA>
+__device__ __forceinline__ void wgmma_n128(float* d, uint64_t ad, uint64_t bd) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate ? 1u : 0u)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, %67, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(ad), "l"(bd), "r"(1), "n"(SA));
 }
 
-// All previously issued MMAs of this thread arrive (once) on `bar` when they complete.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int SA>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t ad, uint64_t bd) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, %19, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(ad), "l"(bd), "r"(1), "n"(SA));
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {   // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <int SA>
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t ad, uint64_t bd) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, %11, 1, 0, 0;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(ad), "l"(bd), "r"(1), "n"(SA));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-
-// ------------------------------------------------------------------------------------------ CTA pairs (cta_group::2)
-// A thread-block cluster of two CTAs can issue one MMA over both SMs: M = 256 (128 rows per CTA, each CTA's own A tile and
-// TMEM), while the N x K B operand is SPLIT — CTA 0's shared memory holds rows [0, N/2), CTA 1's rows [N/2, N) at the same
-// offset — so every SM reads and receives only half of each weight plane.  Issued by one thread of the leader CTA (rank 0).
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// ------------------------------------------------------------------------------------------ accumulator scratch
+// Base of this CTA's [512 columns][128 rows] fp32 scratch; set by the kernel before its first barrier.
+__shared__ float* tm_base;
+__device__ __forceinline__ float* tm_word(uint32_t taddr) {
+  return tm_base + (size_t)(taddr & 0xffffu) * 128 + (taddr >> 16) + (threadIdx.x & 31);
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+// wgmma fragment of an M=64 x N tile (rows 64 wg .. 64 wg + 63 of the scratch, columns col0 ..) <-> scratch
+template <int N>
+__device__ __forceinline__ void acc_store(const float* d, int col0, int wg) {
+  const int lane = threadIdx.x & 31, row = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 2; ++j)
+    tm_base[(size_t)(col0 + 8 * (j >> 2) + 2 * (lane & 3) + (j & 1)) * 128 + row + 8 * ((j >> 1) & 1)] = d[j];
 }
-// shared::cluster address of `p` (a shared::cta pointer of this CTA) in the CTA of rank `cta`
-__device__ __forceinline__ uint32_t mapa_u32(const void* p, uint32_t cta) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_u32(p)), "r"(cta));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// (a plain cp.async.bulk whose mbarrier lives in the OTHER CTA of the pair never completes — tried; only the tensor-map TMA
-// forms have the cta_group::2 variant that signals the leader's barrier — hence the relay lanes of the layer megakernel)
-// same without the release: for pure event forwarding (nothing this thread wrote has to become visible with the arrival)
-__device__ __forceinline__ void mbar_arrive_remote_relaxed(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst, uint32_t ncols) {   // one full warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// instruction descriptor for the pair MMA: M = 256
-__device__ __forceinline__ uint32_t umma_idesc_bf16_m256(int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;
-  d |= 1u << 7;
-  d |= 1u << 10;
-  d |= (uint32_t)(n >> 3) << 17;
-  d |= (uint32_t)(256 >> 4) << 24;
-  return d;
-}
-__device__ __forceinline__ void umma_bf16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate ? 1u : 0u)
-      : "memory");
-}
-// all previously issued pair MMAs of this thread arrive on the mbarrier at this offset in BOTH CTAs (mask 0b11)
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"((unsigned short)3)
-               : "memory");
+template <int N>
+__device__ __forceinline__ void acc_load(float* d, int col0, int wg) {
+  const int lane = threadIdx.x & 31, row = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 2; ++j)
+    d[j] = tm_base[(size_t)(col0 + 8 * (j >> 2) + 2 * (lane & 3) + (j & 1)) * 128 + row + 8 * ((j >> 1) & 1)];
 }
 
-// TMEM -> registers: this thread's lane (32*(warp%4) + laneid), `N` consecutive 32-bit columns from taddr.
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-// Asynchronous variants: issue several loads / stores back to back, then ONE wait (tcgen05.wait covers all
-// previously issued operations of the thread), instead of paying the TMEM round trip once per instruction.
+// scratch -> registers: this thread's row (32*(warp%4) + laneid, encoded in taddr's upper half), `N` consecutive columns
 __device__ __forceinline__ void tmem_ld8_nw(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
+  const float* p = tm_word(taddr);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) r[i] = __float_as_uint(p[i * 128]);
 }
 __device__ __forceinline__ void tmem_ld32_nw(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+  const float* p = tm_word(taddr);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(p[i * 128]);
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void tmem_ld_wait() {}
+__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
+  const float* p = tm_word(taddr);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = p[i * 128];
+}
+__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
+  const float* p = tm_word(taddr);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] = p[i * 128];
+}
 __device__ __forceinline__ void tmem_st8_nw(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-               "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-               "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
+  float* p = tm_word(taddr);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) p[i * 128] = v[i];
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// N x 8 columns in one go
+__device__ __forceinline__ void tmem_st_wait() {}
 template <int N8>
 __device__ __forceinline__ void tmem_ld8xN(uint32_t taddr, float* v) {
-  uint32_t r[N8 * 8];
+  const float* p = tm_word(taddr);
 #pragma unroll
-  for (int q = 0; q < N8; ++q) tmem_ld8_nw(taddr + q * 8, r + q * 8);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < N8 * 8; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N8 * 8; ++i) v[i] = p[i * 128];
 }
 template <int N8>
-__device__ __forceinline__ void tmem_st8xN(uint32_t taddr, const float* v) {   // caller waits (tmem_st_wait) later
+__device__ __forceinline__ void tmem_st8xN(uint32_t taddr, const float* v) {
 #pragma unroll
   for (int q = 0; q < N8; ++q) tmem_st8_nw(taddr + q * 8, v + q * 8);
 }
-// two 32-column chunks with one wait
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float* v) {
-  uint32_t r[64];
-  tmem_ld32_nw(taddr, r);
-  tmem_ld32_nw(taddr + 32, r + 32);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < 64; ++i) v[i] = __uint_as_float(r[i]);
-}
+__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float* v) { tmem_ld8xN<8>(taddr, v); }
+__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) { tmem_st8_nw(taddr, v); }
+// Ordering of scratch accesses between threads is given by the CTA barriers around them; these mark the places.
+__device__ __forceinline__ void tc_fence_before() {}
+__device__ __forceinline__ void tc_fence_after() {}
 
-// registers -> TMEM (per-thread scratch columns)
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr),
-               "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-               "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])),
-               "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7]))
-               : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
+// The packed fp32x2 intrinsics of sm_100 (__fmul2_rn & co.) are not available when compiling device code for sm_90:
+// two-lane versions with the same names, one instruction per lane (the host pass sees the toolkit's declarations).
+#if defined(__CUDA_ARCH__) && __CUDA_ARCH__ < 1000
+__device__ __forceinline__ float2 __fmul2_rn(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ float2 __fadd2_rn(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 __ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+#endif
 
 // fast activations for the tensor path (one MUFU each; operands are rounded to bf16 anyway)
 __device__ __forceinline__ float tanh_fast(float x) {
@@ -235,7 +172,7 @@ __device__ __forceinline__ float tanh_fast(float x) {
 __device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
 __device__ __forceinline__ float silu_fast(float x) { return x * sigmoid_fast(x); }
 
-// packed fp32x2 versions (FFMA2 / FMUL2 / FADD2 on sm_100a: two lanes per issued instruction)
+// packed fp32x2 versions (two lanes per call)
 __device__ __forceinline__ float2 sigmoid_fast2(float2 x) {
   const float2 hx = __fmul2_rn(x, make_float2(0.5f, 0.5f));
   const float2 t = make_float2(tanh_fast(hx.x), tanh_fast(hx.y));
@@ -252,24 +189,11 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(h);
 }
 
-
-// 64-bit UMMA shared-memory descriptor for a K-major operand WITHOUT swizzle ("interleaved" canonical layout,
-// cute UMMA::LayoutType::SWIZZLE_NONE): core matrices of 8 rows x 16 bytes are contiguous (128 B); consecutive
-// 8-row groups are `sbo` bytes apart, the two 16-byte K chunks of one K=16 step are `lbo` bytes apart.
-__device__ __forceinline__ uint64_t umma_desc_k16(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;
-}
-
 // ------------------------------------------------------------------------------------- split-bf16 operands
 // Every GEMM operand of the tensor path is the pair (hi, lo) of bf16 numbers with hi = RN_bf16(value)
 // and lo = RN_bf16(value - hi): hi + lo carries >= 16 significant bits (relative error
 // <= 2^-18) and is exactly representable in fp32.  A product is evaluated as A_hi.W_hi + A_lo.W_hi + A_hi.W_lo
-// (three tcgen05 MMAs accumulating into the same fp32 TMEM columns; the dropped A_lo.W_lo term is 2^-18 relative).
+// (three wgmma products accumulating into the same fp32 registers; the dropped A_lo.W_lo term is 2^-18 relative).
 __device__ __forceinline__ void split_bf16x2(float a, float b, uint32_t& hi, uint32_t& lo) {
   __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
   hi = *reinterpret_cast<uint32_t*>(&h);

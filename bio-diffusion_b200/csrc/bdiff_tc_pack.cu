@@ -7,10 +7,11 @@ namespace bdiff {
 size_t tc_blob_bytes(int Ed, int Xd) { return tc_edge_stream_bytes(Ed, Xd); }
 size_t tc_node_blob_bytes() { return tc_node_stream_bytes(0); }      // the last layer's stream is shorter
 
-// A layer's stream is [CTA 0's half | CTA 1's half] (the megakernel runs CTA pairs, cta_group::2: an N-row plane is split between
-// the two shared memories, CTA c supplying rows [c N/2, (c+1) N/2) of every MMA's B operand).  Per CTA, in streaming order:
+// A layer's stream is [N half 0 | N half 1]: every N-row weight plane is split in two, half c holding rows [c N/2, (c+1) N/2)
+// (the megakernel streams and multiplies one half at a time, accumulating into D columns of the same range).  Per half, in
+// streaming order:
 // Edge pass:  G0: K0S steps x 128 local rows (W0e rows [128 c, 128 c + 128), zero-padded to K0S*16 K rows)
-//             for k = 1..3:  16 steps x 160 local rows = [W_k rows 128 c .. +128 | 32 gate rows: CTA 0 -> U0, CTA 1 -> U1],
+//             for k = 1..3:  16 steps x 160 local rows = [W_k rows 128 c .. +128 | 32 gate rows: half 0 -> U0, half 1 -> U1],
 //                            2 steps x 128 local rows (W_k K rows 256..287)
 //             G4: 16 steps x 16 local rows (Wg_3 rows [16 c, 16 c + 16))
 // Gate rows: GCP kk = gi + 1 adds +Wg_{kk-1} m_{kk-1} to U[(kk-1) & 1] and starts U[kk & 1] = -Wg_kk m_{kk-1} (sign folded into

@@ -1,5 +1,5 @@
 /*
- * bdiff.h — C ABI of libbdiff_sm100.so: the B200-native GCPNet denoiser hot path of GCDM.
+ * bdiff.h — C ABI of libbdiff_sm90.so: the H100-native GCPNet denoiser hot path of GCDM.
  *
  * The reference (BioinfoMachineLearning/bio-diffusion) has no FFI for this path; its seam is the Python
  * class contract `dynamics_network.forward(batch, xh, t) -> (batch, net_out)` selected in
@@ -40,8 +40,8 @@ extern "C" {
 #endif
 
 /* Compute modes.  PARITY: every multiply-add in fp32 FFMA (differs from the reference only by
- * summation order).  TENSOR: the per-edge message GEMMs run on tcgen05 tensor cores
- * (operands rounded to the tensor format, fp32 accumulation in TMEM). */
+ * summation order).  TENSOR: the dense GEMMs of the layers run on the tensor cores (wgmma) with split-bf16
+ * operands and fp32 accumulation. */
 #define BDIFF_MODE_PARITY_FP32 0
 #define BDIFF_MODE_TENSOR 1
 
@@ -84,16 +84,11 @@ BDIFF_API int32_t bdiff_weights_missing(const bdiff_handle* h);
 BDIFF_API int32_t bdiff_prepare(bdiff_handle* h, void* stream);
 
 /* Hardware self test of the split-bf16 machinery of the tensor mode (csrc/bdiff_selftest.cu): hi/lo A blocks,
- * un-swizzled K=16 weight slabs, three (variant bit 1: four, node-tile row views) products per K step, TMEM pair
- * exchange.  C[128,336] <- [A W^T (320 cols; the last 32 negated) | exchange (16 cols)] for A fp32[128,128],
- * W fp32[320,128] (device pointers).  variant bit 0 swaps LBO/SBO (must then FAIL the comparison).  Synchronises. */
+ * un-swizzled K=16 weight slabs, three (variant bit 1: four, node-tile row views) products per K step, accumulator
+ * scratch pair exchange.  C[128,336] <- [A W^T (320 cols; the last 32 negated) | exchange (16 cols)] for
+ * A fp32[128,128], W fp32[320,128] (device pointers).  Synchronises. */
 BDIFF_API int32_t bdiff_selftest_split(void* stream, int32_t variant, const float* A, const float* W, float* C);
 
-/* Hardware self test of the CTA-pair (cta_group::2) machinery: a two-CTA cluster, TMEM allocated for the pair, every weight
- * plane split between the two shared memories, the peer's TMA completion relayed by a remote mbarrier arrive, one commit
- * multicast to both CTAs.  C[256,320] <- A W^T for A fp32[256,128], W fp32[320,128] (device pointers), split-bf16 operands.
- * Synchronises. */
-BDIFF_API int32_t bdiff_selftest_pair(void* stream, const float* A, const float* W, float* C);
 
 /* Replaces: GCPNetDynamics.get_fully_connected_edge_index (gcpnet.py:1054-1066) — as an implicit plan.
  * batch_index int64[N] (sorted molecule ids, as every caller provides), mask uint8[N].  Builds the

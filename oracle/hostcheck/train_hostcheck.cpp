@@ -1,4 +1,4 @@
-// train_hostcheck.cpp — TEST INFRASTRUCTURE ONLY (never linked into libbdiff_sm100.so, never on the product path).
+// train_hostcheck.cpp — TEST INFRASTRUCTURE ONLY (never linked into libbdiff_sm90.so, never on the product path).
 //
 // Compiles the product's training pass (bio-diffusion_b200/csrc/bdiff_train_engine.cuh: the functors every CUDA kernel
 // of bdiff_train.cu executes and the orchestration of the GEMMs between them) against a host backend — plain loops and

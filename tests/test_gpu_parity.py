@@ -31,7 +31,7 @@ def relerr(a, b):
 def test_library_loaded_is_in_tree():
     import bdiff
     lib = bdiff.load_library()
-    assert "bio-diffusion_b200/bdiff/libbdiff_sm100.so" in lib._name
+    assert "bio-diffusion_b200/bdiff/libbdiff_sm90.so" in lib._name
 
 
 def test_edge_index_kat_bit_exact():

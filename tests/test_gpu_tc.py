@@ -1,8 +1,8 @@
-"""GPU tests of the tensor-core (tcgen05) path = `mode="tensor"`, the mode bench.py times.
+"""GPU tests of the tensor-core (wgmma) path = `mode="tensor"`, the mode bench.py times.
 
 Arithmetic of that mode: every dense GEMM runs on the 5th-gen tensor cores with SPLIT-bf16 operands — activations and
 weights are each the sum of two bf16 numbers (>= 16 significant bits), products evaluated as
-A_hi.W_hi + A_lo.W_hi + A_hi.W_lo with fp32 accumulation in TMEM — and ex2/rcp activations (~2 ulp).  Stated
+A_hi.W_hi + A_lo.W_hi + A_hi.W_lo with fp32 accumulation — and ex2/rcp activations (~2 ulp).  Stated
 tolerances (the reference's arithmetic is fp32, configs/trainer/default.yaml:15-16):
   * hardware self test vs an fp64 matmul: 3e-5 relative (plain bf16 operands: 2.4e-3);
   * one denoiser forward vs the reference golden output: max-abs <= 1e-4 * max(1, |ref|) on all six fixtures
@@ -41,14 +41,14 @@ def test_umma_selftest_split_matches_fp64_matmul(variant):
     assert rc == 0
     aa = a.double()
     if variant & 2:
-        aa = aa[:32].repeat(4, 1)        # every TMEM lane quarter holds the complete product of the 32 rows
+        aa = aa[:32].repeat(4, 1)        # every row quarter holds the complete product of the 32 rows
     ref = aa @ w.double().t()
     ref[:, 288:] = -ref[:, 288:]
     err = (c[:, :320].double() - ref).abs().max().item() / ref.abs().max().item()
     print(f"split-bf16 UMMA self test variant {variant}: rel err vs fp64 {err:.3e}")
     assert err < 3e-5, f"UMMA self test rel err {err:.3e}"
     r = torch.arange(128, device="cuda", dtype=torch.float32)[:, None] * 8 + torch.arange(8, device="cuda")[None, :]
-    assert torch.equal(c[:, 320:328], 1000 + r) and torch.equal(c[:, 328:336], r)      # TMEM pair exchange
+    assert torch.equal(c[:, 320:328], 1000 + r) and torch.equal(c[:, 328:336], r)      # accumulator-scratch pair exchange
 
 
 def make_net(cname, seed, mode, scale=1.0):

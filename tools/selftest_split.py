@@ -1,4 +1,4 @@
-"""GPU: run the split-bf16 tcgen05 self test for every variant and print the error against an fp64 matmul."""
+"""GPU: run the split-bf16 wgmma self test for every variant and print the error against an fp64 matmul."""
 import ctypes as C
 import sys, os
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "bio-diffusion_b200"))
@@ -9,7 +9,7 @@ lib = bdiff.load_library()
 g = torch.Generator().manual_seed(0)
 a = torch.randn((128, 128), generator=g).cuda()
 w = torch.randn((320, 128), generator=g).cuda()
-for variant in (0, 2):      # bit 0 (LBO/SBO swapped) reads outside shared memory: verified to fault, not run
+for variant in (0, 2):
     c = torch.zeros((128, 336), device="cuda")
     rc = lib.bdiff_selftest_split(C.c_void_p(torch.cuda.current_stream().cuda_stream), variant, C.c_void_p(a.data_ptr()),
                                   C.c_void_p(w.data_ptr()), C.c_void_p(c.data_ptr()))

@@ -48,6 +48,8 @@ PROTOTYPES = {
     "bdiff_decode_z0": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p]),
     "bdiff_center_noise": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bdiff_repaint_combine": (C.c_int32, [C.c_void_p] * 9),
+    "bdiff_renoise": (C.c_int32, [C.c_void_p] * 7),
     "bdiff_check": (C.c_int32, [C.c_void_p, C.c_void_p]),
     "bdiff_check_stability": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32, C.c_int32] + [C.c_void_p] * 3 + [C.c_float] * 3 +
                               [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),

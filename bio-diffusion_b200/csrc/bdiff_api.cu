@@ -772,6 +772,30 @@ int32_t bdiff_center_noise(bdiff_handle* h, void* stream, const float* noise_x, 
   return e == cudaSuccess ? BDIFF_OK : h->fail(BDIFF_ECUDA, "center_noise: %s", cudaGetErrorString(e));
 }
 
+int32_t bdiff_repaint_combine(bdiff_handle* h, void* stream, float* z, const float* xh0, const uint8_t* fixed,
+                              const float* noise_x, const float* noise_h, const float* known_table,
+                              const int32_t* op_index) {
+  if (!h || !z || !xh0 || !fixed || !noise_x || !noise_h || !known_table || !op_index)
+    return h ? h->fail(BDIFF_EINVAL, "null argument") : BDIFF_EINVAL;
+  if (!h->have_plan) return h->fail(BDIFF_ESTATE, "no topology plan");
+  launch_repaint_combine(static_cast<cudaStream_t>(stream), h->plan, h->d, z, xh0, fixed, noise_x, noise_h, known_table,
+                         op_index);
+  h->launches++;
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? BDIFF_OK : h->fail(BDIFF_ECUDA, "repaint_combine: %s", cudaGetErrorString(e));
+}
+
+int32_t bdiff_renoise(bdiff_handle* h, void* stream, float* z, const float* noise_x, const float* noise_h,
+                      const float* jump_table, const int32_t* jump_index) {
+  if (!h || !z || !noise_x || !noise_h || !jump_table || !jump_index)
+    return h ? h->fail(BDIFF_EINVAL, "null argument") : BDIFF_EINVAL;
+  if (!h->have_plan) return h->fail(BDIFF_ESTATE, "no topology plan");
+  launch_step(static_cast<cudaStream_t>(stream), h->plan, h->d, 3, z, nullptr, noise_x, noise_h, jump_table, jump_index, z);
+  h->launches++;
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? BDIFF_OK : h->fail(BDIFF_ECUDA, "renoise: %s", cudaGetErrorString(e));
+}
+
 int32_t bdiff_check(bdiff_handle* h, void* stream) {
   if (!h) return BDIFF_EINVAL;
   cudaError_t e = cudaStreamSynchronize(static_cast<cudaStream_t>(stream));

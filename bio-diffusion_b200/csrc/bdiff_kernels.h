@@ -49,6 +49,9 @@ void launch_finalize(cudaStream_t st, const Plan& p, const Dims& d, const Work& 
 void launch_step(cudaStream_t st, const Plan& p, const Dims& d, int mode, const float* z, const float* eps,
                  const float* noise_x, const float* noise_h, const float* coef_table, const int* step_ptr,
                  float* out);
+void launch_repaint_combine(cudaStream_t st, const Plan& p, const Dims& d, float* z, const float* xh0,
+                            const uint8_t* fixed, const float* noise_x, const float* noise_h,
+                            const float* known_table, const int* op_ptr);
 void launch_edge_index(cudaStream_t st, const Plan& p, long long* out);
 void launch_edge_rc(cudaStream_t st, const Plan& p, int4* out, long long n);
 // one slice of a reference parameter tensor -> kernel layout (see k_pack_multi)

@@ -811,6 +811,8 @@ __global__ void __launch_bounds__(128) k_finalize(Plan p, Dims d, Work w, float*
 //   z' = z / alpha_ts - c_eps * eps + sigma * noise_mc ; x-part of z' re-centred.          coef = {alpha_ts, c_eps, sigma, t}
 // mode 1 (decode, :559-577,880-885): out = inv_alpha0 * (z - sigma0 * eps) + sigma_x * noise_mc.  coef = {inv_alpha0, sigma0, sigma_x, 0}
 // mode 2: out = noise_mc (z_T).   noise_mc = raw randn masked, x-part centred per molecule (:795-819).
+// mode 3 (jump back of inpaint, sample_p_zt_given_zs :1163-1201 indexing alpha_t|s by batch_index):
+//   z' = alpha_t|s * z + sigma_t|s * noise_mc ; x-part of z' re-centred.                coef = {alpha_t|s, sigma_t|s, s, t}
 __global__ void __launch_bounds__(128) k_step(Plan p, Dims d, int mode, const float* __restrict__ z,
                                               const float* __restrict__ eps, const float* __restrict__ noise_x,
                                               const float* __restrict__ noise_h,
@@ -845,12 +847,13 @@ __global__ void __launch_bounds__(128) k_step(Plan p, Dims d, int mode, const fl
       float v;
       if (mode == 0) v = z[(size_t)i * ld + c] / c0 - c1 * eps[(size_t)i * ld + c] + c2 * nz;
       else if (mode == 1) v = c0 * (z[(size_t)i * ld + c] - c1 * eps[(size_t)i * ld + c]) + c2 * nz;
+      else if (mode == 3) v = c0 * z[(size_t)i * ld + c] + c1 * nz;
       else v = nz;
       out[(size_t)i * ld + c] = v;
       if (c < 3) t[c] += v;
     }
   }
-  if (mode != 0) return;
+  if (mode == 1 || mode == 2) return;
   block_sum4(t, red);
   const float zx = cnt > 0.f ? t[0] / cnt : 0.f, zy = cnt > 0.f ? t[1] / cnt : 0.f, zz = cnt > 0.f ? t[2] / cnt : 0.f;
   for (int i = n0 + threadIdx.x; i < n1; i += 128) {
@@ -858,6 +861,66 @@ __global__ void __launch_bounds__(128) k_step(Plan p, Dims d, int mode, const fl
     out[(size_t)i * ld + 0] -= zx * m;
     out[(size_t)i * ld + 1] -= zy * m;
     out[(size_t)i * ld + 2] -= zz * m;
+  }
+}
+
+// One CTA per molecule: the RePaint combination of inpaint (variational_diffusion.py:1659-1667, 1694-1713), applied after
+// the reverse step has written z_unknown into z.  known = {alpha_s, sigma_s} = known_table[2 * *op_ptr]:
+//   z_known = alpha_s * xh0 + sigma_s * noise_mc                      (compute_noised_representation, :910-931)
+//   z_known.x += mean_fixed(z_unknown.x) - mean_fixed(z_known.x)      (per molecule)
+//   z[fixed rows] = z_known                                           (z[free rows] stays z_unknown)
+// A molecule without fixed atoms is left untouched.  Fixed-order reductions: the result is bit-reproducible.
+__global__ void __launch_bounds__(128) k_repaint_combine(Plan p, Dims d, float* __restrict__ z,
+                                                         const float* __restrict__ xh0,
+                                                         const uint8_t* __restrict__ fixed,
+                                                         const float* __restrict__ noise_x,
+                                                         const float* __restrict__ noise_h,
+                                                         const float* __restrict__ known_table,
+                                                         const int* __restrict__ op_ptr) {
+  __shared__ float red[4][4];
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const int ld = 3 + d.F;
+  const int op = __ldg(op_ptr);
+  const float alpha = __ldg(known_table + 2 * op), sigma = __ldg(known_table + 2 * op + 1);
+  // 1) centre of the raw x noise over the molecule's present atoms
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float m = p.mask[i] ? 1.f : 0.f;
+    s[0] += noise_x[(size_t)i * 3 + 0] * m;
+    s[1] += noise_x[(size_t)i * 3 + 1] * m;
+    s[2] += noise_x[(size_t)i * 3 + 2] * m;
+    s[3] += m;
+  }
+  block_sum4(s, red);
+  const float cnt = s[3];
+  const float nc[3] = {cnt > 0.f ? s[0] / cnt : 0.f, cnt > 0.f ? s[1] / cnt : 0.f, cnt > 0.f ? s[2] / cnt : 0.f};
+  // 2) sums over the fixed atoms of z_unknown.x and of z_known.x
+  float u[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    if (!fixed[i]) continue;
+    const float m = p.mask[i] ? 1.f : 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      u[c] += z[(size_t)i * ld + c];
+      q[c] += alpha * xh0[(size_t)i * ld + c] + sigma * ((noise_x[(size_t)i * 3 + c] - nc[c] * m) * m);
+    }
+    u[3] += 1.f;
+  }
+  block_sum4(u, red);
+  block_sum4(q, red);
+  const float nf = u[3];
+  if (nf == 0.f) return;                                 // no fixed atom: the molecule is sampled freely
+  const float sh[3] = {u[0] / nf - q[0] / nf, u[1] / nf - q[1] / nf, u[2] / nf - q[2] / nf};
+  // 3) overwrite the fixed rows
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    if (!fixed[i]) continue;
+    const float m = p.mask[i] ? 1.f : 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      z[(size_t)i * ld + c] = (alpha * xh0[(size_t)i * ld + c] + sigma * ((noise_x[(size_t)i * 3 + c] - nc[c] * m) * m)) + sh[c];
+    for (int f = 0; f < d.F; ++f)
+      z[(size_t)i * ld + 3 + f] = alpha * xh0[(size_t)i * ld + 3 + f] + sigma * (noise_h[(size_t)i * d.F + f] * m);
   }
 }
 
@@ -952,6 +1015,11 @@ void launch_step(cudaStream_t st, const Plan& p, const Dims& d, int mode, const 
                  const float* noise_x, const float* noise_h, const float* coef_table, const int* step_ptr,
                  float* out) {
   k_step<<<p.B, 128, 0, st>>>(p, d, mode, z, eps, noise_x, noise_h, coef_table, step_ptr, out);
+}
+void launch_repaint_combine(cudaStream_t st, const Plan& p, const Dims& d, float* z, const float* xh0,
+                            const uint8_t* fixed, const float* noise_x, const float* noise_h,
+                            const float* known_table, const int* op_ptr) {
+  k_repaint_combine<<<p.B, 128, 0, st>>>(p, d, z, xh0, fixed, noise_x, noise_h, known_table, op_ptr);
 }
 void launch_edge_index(cudaStream_t st, const Plan& p, long long* out) {
   if (p.E > 0) k_edge_index<<<(unsigned)((p.E + 255) / 256), 256, 0, st>>>(p, out);

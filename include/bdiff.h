@@ -144,6 +144,25 @@ BDIFF_API int32_t bdiff_decode_z0(bdiff_handle* h, void* stream, const float* z0
 BDIFF_API int32_t bdiff_center_noise(bdiff_handle* h, void* stream, const float* noise_x, const float* noise_h,
                                      float* z);
 
+/* Replaces: the RePaint combination inside EquivariantVariationalDiffusion.inpaint (variational_diffusion.py:1659-1667,
+ * 1694-1713), run after bdiff_reverse_step has turned z into z_unknown:
+ *   z_known = alpha_s*xh0 + sigma_s*noise (compute_noised_representation, :910-931: noise masked, x-part centred over the
+ *   molecule);  z_known.x += mean over fixed atoms of (z_unknown.x - z_known.x), per molecule;  z[fixed] = z_known.
+ * xh0 fp32[N,3+F] (the input molecule, x centred on its fixed atoms), fixed uint8[N] (1 = atom held fixed), noise_x
+ * fp32[N,3] / noise_h fp32[N,F] the two RAW randn draws of the known part.  known_table: DEVICE rows {alpha_s, sigma_s};
+ * the row used is known_table[2 * *op_index] (op_index: DEVICE int32), so the call can sit in a replayed CUDA graph.
+ * z is updated in place; rows of free atoms and all rows of a molecule without fixed atoms are left unchanged. */
+BDIFF_API int32_t bdiff_repaint_combine(bdiff_handle* h, void* stream, float* z, const float* xh0, const uint8_t* fixed,
+                                        const float* noise_x, const float* noise_h, const float* known_table,
+                                        const int32_t* op_index);
+
+/* Replaces: sample_p_zt_given_zs (variational_diffusion.py:1163-1201; alpha_t|s taken per molecule, i.e. indexed by
+ * batch_index where :1177 indexes it by node_mask), the jump back of inpaint (:1730-1749):
+ *   z' = alpha_t|s*z + sigma_t|s*noise (noise masked, x-part centred);  z'[:, :3] re-centred.
+ * jump_table: DEVICE rows {alpha_t|s, sigma_t|s, s, t}; row jump_table[4 * *jump_index] (DEVICE int32).  In place. */
+BDIFF_API int32_t bdiff_renoise(bdiff_handle* h, void* stream, float* z, const float* noise_x, const float* noise_h,
+                                const float* jump_table, const int32_t* jump_index);
+
 /* Synchronises `stream` and reports deferred device-side conditions of the work issued so far on this handle.
  * Today: the tile scheduler of the all-layers tensor-core kernel (replaces the kernel boundaries between
  * GCPInteractions layers, gcpnet.py:1161-1176) raises a flag if a dependency wait ever times out; that is an internal

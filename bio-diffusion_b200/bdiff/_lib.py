@@ -64,7 +64,6 @@ PROTOTYPES = {
     "bdiff_param_floats": (C.c_int64, [C.c_void_p]),
     "bdiff_param_layout": (C.c_int32, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "bdiff_train_precision": (C.c_int32, [C.c_void_p, C.c_int32]),
-    "bdiff_train_variant": (C.c_int32, [C.c_void_p, C.c_int32]),
     "bdiff_train_timing": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_char_p, C.c_int64]),
     "bdiff_train_forward": (C.c_int32, [C.c_void_p] * 7),
     "bdiff_train_backward": (C.c_int32, [C.c_void_p] * 4),

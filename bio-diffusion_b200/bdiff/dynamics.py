@@ -19,7 +19,6 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-import os
 from typing import Any, Dict, Optional, Tuple
 
 import torch
@@ -123,9 +122,6 @@ class GCPNetDynamicsB200(nn.Module):
         if rc != 0:
             raise _lib.BdiffError(f"bdiff_create failed (code {rc}): {lib.bdiff_last_error(None).decode()}")
         self._handle = h
-        variant = os.environ.get("BDIFF_TRAIN_VARIANT")
-        if variant is not None:
-            _lib.check(h, lib.bdiff_train_variant(h, int(variant)), "bdiff_train_variant")
         return h
 
     def __del__(self):
@@ -327,12 +323,6 @@ class GCPNetDynamicsB200(nn.Module):
                       context: Optional[torch.Tensor] = None, num_mols: Optional[int] = None) -> torch.Tensor:
         """`denoise` with a grad_fn: fp32 training pass of the library (one tape at a time)."""
         return _DenoiseTrainFn.apply(self, batch_index, mask, xh, t, context, num_mols, *self.parameters())
-
-    def set_train_variant(self, variant: int) -> None:
-        """1 (default): split message GCP 0 + tape-resident activations; 0: the reference's operator graph one to one (same
-        mathematics, more FLOPs and bytes; the cross-check).  Takes effect at the next training forward."""
-        lib = _lib.load()
-        _lib.check(self._ensure_handle(), lib.bdiff_train_variant(self._ensure_handle(), int(variant)), "bdiff_train_variant")
 
     def set_train_precision(self, tf32: bool) -> None:
         """GEMMs of the training pass: fp32 (default) or TF32 tensor cores."""

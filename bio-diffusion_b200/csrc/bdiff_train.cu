@@ -99,7 +99,6 @@ struct TrainState {
   const float* params = nullptr;
   float* grads = nullptr;
   bool tf32 = false;
-  int variant = 1, laid_variant = -1;    // 1 = split message GCP 0 (default since it was validated on the device); 0 = plain graph
 };
 
 void train_destroy(TrainState* t) {
@@ -125,9 +124,7 @@ int32_t ensure_train(bdiff_handle* h, cudaStream_t st, const float* params, floa
   }
   cublasSetStream(t->be.cb, st);
   t->be.st = st;
-  if (t->plan_epoch == h->plan_epoch && t->params == params && (grads == nullptr || t->grads == grads) &&
-      t->laid_variant == t->variant)
-    return BDIFF_OK;
+  if (t->plan_epoch == h->plan_epoch && t->params == params && (grads == nullptr || t->grads == grads)) return BDIFF_OK;
   train::NetDims d{h->d.F, h->d.C, h->d.Hin, h->d.Ed, h->d.Xd, h->d.L};
   train::Topo tp;
   const Plan& p = h->plan;
@@ -141,9 +138,7 @@ int32_t ensure_train(bdiff_handle* h, cudaStream_t st, const float* params, floa
     if (it == h->param_layout.end()) { ++missing; return train::ParamRef{params, g}; }
     return train::ParamRef{params + it->second.first, g ? g + it->second.first : nullptr};
   };
-  const bool same_shape = t->plan_epoch == h->plan_epoch && t->laid_variant == t->variant;
-  t->eng.variant = t->variant;
-  t->laid_variant = t->variant;
+  const bool same_shape = t->plan_epoch == h->plan_epoch;
   if (!same_shape) {
     const size_t need = t->eng.layout(d, tp, nullptr, look);
     if (missing) return h->fail(BDIFF_ESTATE, "internal: %d parameter names unknown to the training pass", missing);
@@ -246,14 +241,6 @@ int32_t bdiff_train_timing(bdiff_handle* h, void* stream, int32_t enable, char* 
   return BDIFF_OK;
 }
 
-int32_t bdiff_train_variant(bdiff_handle* h, int32_t variant) {
-  if (!h) return BDIFF_EINVAL;
-  if (variant != 0 && variant != 1) return h->fail(BDIFF_EINVAL, "training variant must be 0 or 1");
-  if (!h->train) h->train = new TrainState();
-  h->train->variant = variant;
-  return BDIFF_OK;
-}
-
 int32_t bdiff_train_forward(bdiff_handle* h, void* stream, const float* params_flat, const float* xh, const float* t,
                             const float* context, float* net_out) {
   if (!h || !params_flat || !xh || !t || !net_out) return h ? h->fail(BDIFF_EINVAL, "null argument") : BDIFF_EINVAL;
@@ -267,7 +254,7 @@ int32_t bdiff_train_forward(bdiff_handle* h, void* stream, const float* params_f
 
 int32_t bdiff_train_backward(bdiff_handle* h, void* stream, const float* d_net_out, float* grads_flat) {
   if (!h || !d_net_out || !grads_flat) return h ? h->fail(BDIFF_EINVAL, "null argument") : BDIFF_EINVAL;
-  if (!h->train || !h->train->eng.have_tape || h->train->plan_epoch != h->plan_epoch || h->train->laid_variant != h->train->variant)
+  if (!h->train || !h->train->eng.have_tape || h->train->plan_epoch != h->plan_epoch)
     return h->fail(BDIFF_ESTATE, "bdiff_train_backward needs the tape of a bdiff_train_forward on the current plan");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   TrainState* t = h->train;

@@ -8,6 +8,10 @@
 // (vector_down / vector_down_frames / scalar_out / vector_up / vector_out_scale and their two transposes) with small
 // element-wise kernels between them, plus gather / segmented-sum kernels that use the implicit edge plan (edges of a
 // molecule are its nact x nact block, row-major), so no scatter ever needs an atomic: every sum runs in a fixed order.
+// Two departures from the graph, same mathematics: message GCP 0 runs in the sampler's split form (the endpoint blocks
+// of scalar_out are node-level GEMMs PI = h.Wsi^T, PJ = h.Wsj^T, gathered per edge, instead of an [E, 512+Ed] gather
+// and GEMM), and the backward writes every input gradient straight into its consumer (beta = 1 into the residual
+// stream) with the activations act1(z) and silu(z1) read from the tape.
 //
 // The file is written against a small `Backend` concept  { run(n, functor); gemm(...); }  so that the very same
 // functors and the very same orchestration compile twice: with the CUDA backend of bdiff_train.cu (kernels + cuBLAS
@@ -235,7 +239,6 @@ struct FDVecOut {       // d gate (pre-sigmoid) and d up from d v_out
     dgate[idx] = acc * g * (1.0f - g);
   }
 };
-struct FAct { const float* z; float* a; int act; BDT_HD void operator()(long long i) const { a[i] = t_act(act, z[i]); } };
 struct FDZ {            // dz = ds_out * act0'(z) + dgz * act1'(z)
   const float* ds; int ld_ds; const float* dgz; const float* z; int n, act0, act1; float* dz;
   BDT_HD void operator()(long long idx) const {
@@ -249,11 +252,11 @@ struct FDZ {            // dz = ds_out * act0'(z) + dgz * act1'(z)
 };
 struct FMulDSilu { float* d; const float* z; BDT_HD void operator()(long long i) const { d[i] *= t_dact(1, z[i]); } };
 struct FDNorm {         // dhid (+)= dvnorm / sqrt(sum hid^2 + 1e-8) * hid
-  const float* dmerged; int fan, S_in, H; const float* hid; float* dhid; int accumulate;
+  const float* dvq; int ld, H; const float* hid; float* dhid; int accumulate;
   BDT_HD void operator()(long long idx) const {
     const long long m = idx / H; const int h = (int)(idx % H);
     const float a = hid[(m * 3 + 0) * H + h], b = hid[(m * 3 + 1) * H + h], c = hid[(m * 3 + 2) * H + h];
-    const float s = dmerged[m * fan + S_in + h] / sqrtf(a * a + b * b + c * c + 1e-8f);
+    const float s = dvq[m * ld + h] / sqrtf(a * a + b * b + c * c + 1e-8f);
     if (accumulate) {
       dhid[(m * 3 + 0) * H + h] += s * a; dhid[(m * 3 + 1) * H + h] += s * b; dhid[(m * 3 + 2) * H + h] += s * c;
     } else {
@@ -262,10 +265,10 @@ struct FDNorm {         // dhid (+)= dvnorm / sqrt(sum hid^2 + 1e-8) * hid
   }
 };
 struct FDQ {            // dvdf[m,x,c] = sum_a dq[m,c,a] * frames[m,a,x]
-  const float* dmerged; int fan, off; const float* frames; float* dvdf;
+  const float* dvq; int ld, off; const float* frames; float* dvdf;
   BDT_HD void operator()(long long idx) const {
     const long long m = idx / 9; const int x = (int)(idx % 9) / 3, c = (int)(idx % 3);
-    const float* dq = dmerged + m * fan + off + c * 3;
+    const float* dq = dvq + m * ld + off + c * 3;
     const float* f = frames + m * 9;
     dvdf[idx] = dq[0] * f[0 + x] + dq[1] * f[3 + x] + dq[2] * f[6 + x];
   }
@@ -292,18 +295,6 @@ struct FColsum2 {
 };
 
 // ------------------------------------------------------------------------------------------------ functors: message passing
-struct FGatherS {       // merged0[:, :512+Ed] = [h[row] | e | h[col]]                (gcpnet.py:694)
-  const EdgeRc* rc; const float* h; int ld_h; const float* e; int Ed; float* out; int fan;
-  BDT_HD void operator()(long long idx) const {
-    const int w = 512 + Ed;
-    const long long ed = idx / w; const int j = (int)(idx % w);
-    float v;
-    if (j < 256) v = h[(long long)rc[ed].row * ld_h + j];
-    else if (j < 256 + Ed) v = e[ed * Ed + (j - 256)];
-    else v = h[(long long)rc[ed].col * ld_h + (j - 256 - Ed)];
-    out[ed * fan + j] = v;
-  }
-};
 struct FGatherV {       // mv_t = [chi[row] | xi | chi[col]]
   const EdgeRc* rc; const float* chi; int ld_c; const float* xi; int Xd; float* out;
   BDT_HD void operator()(long long idx) const {
@@ -379,21 +370,6 @@ struct FGatherRowV {    // dv[e] = da_v[row]
     const long long ex = idx / 32; const int o = (int)(idx % 32);
     const long long e = ex / 3; const int x = (int)(ex % 3);
     dv[idx] = dav[((long long)rc[e].row * 3 + x) * ld + o];
-  }
-};
-struct FScatterS {      // dh[n] += sum_row dms[e, :256] + sum_col dms[e, 256+Ed:]
-  Topo tp; const int* apos; const float* dms; int fan, Ed; float* dh; int ld;
-  BDT_HD void operator()(long long idx) const {
-    const long long n = idx / 256; const int j = (int)(idx % 256);
-    long long e0; int na;
-    row_span(tp, apos, n, e0, na);
-    if (na == 0) return;
-    float acc = 0.f;
-    for (int b = 0; b < na; ++b) acc += dms[(e0 + b) * fan + j];
-    const int a = apos[n];
-    const long long base = e0 - (long long)a * na;      // first edge of the molecule
-    for (int r = 0; r < na; ++r) acc += dms[(base + (long long)r * na + a) * fan + 256 + Ed + j];
-    dh[n * ld + j] += acc;
   }
 };
 struct FScatterV {
@@ -481,28 +457,26 @@ struct Gcp {
   float* vt = nullptr; int ldv = 0;    // input vectors [M*3, ldv]
   float* merged = nullptr; int fan = 0; // [M, fan] = [s | vnorm | q]; the scalar_out weight block that multiplies it starts at
   int fanW = 0, wcol = 0;               // column wcol of Ws, whose rows are fanW long (fanW = fan, wcol = 0 unless split)
-  // split form of message GCP 0 (variant 1): merged = [vnorm | q] only; z also gets e.We^T (a second GEMM) and the
-  // node-level projections PI[row] + PJ[col] (gathered in FScalarOut)
+  // split form of message GCP 0: merged = [vnorm | q] only; z also gets e.We^T (a second GEMM) and the node-level
+  // projections PI[row] + PJ[col] (gathered in FScalarOut)
   int split = 0, Ed = 0;
   const float *ee = nullptr, *pi = nullptr, *pj = nullptr; const EdgeRc* rc = nullptr;
-  float *a1t = nullptr, *aff = nullptr;  // variant 1: act1(z) and silu(z1) kept on the tape instead of recomputed
+  float *a1t = nullptr, *aff = nullptr;  // act1(z) (if V_out) and silu(z1) (if ff), kept on the tape for the backward
   float *hid = nullptr, *vdf = nullptr, *z1 = nullptr, *z = nullptr, *up = nullptr, *sg = nullptr;
   const float* frames = nullptr;        // [M, 9]: edge frames or the nodes' mean row frames
 };
 
 struct Scratch {        // sized for the largest entity count; used inside one GCP forward / backward only
-  float *a1, *dz, *dgz, *dg, *dup, *dhid, *dvdf, *part;
+  float *dz, *dgz, *dg, *dup, *dhid, *dvdf, *part;
 };
 
 struct ParamRef { const float* w; float* g; };
 
-// Where a GCP's backward puts its input gradients.  Variant 0: `dmerged` [M, fan] gets d[s | vnorm | q] from one GEMM.
-// Variant 1 (`dvq` set): d s goes straight to its consumer (`ds_dst`, = or +=, skipped when null) and only d[vnorm | q]
-// [M, H+9] is materialised.
+// Where a GCP's backward puts its input gradients: d s into `ds_dst` [M, ld_ds] and d v into `dvt` [M*3, ld_dvt], each
+// as C = grad + beta * C (so beta = 1 accumulates into a residual stream) and skipped when null.  d[vnorm | q] only
+// passes through the engine's DVQ scratch.
 struct BwdOut {
-  float* dmerged = nullptr;
   float* ds_dst = nullptr; int ld_ds = 0; float beta_ds = 0.f;
-  float* dvq = nullptr;
   float* dvt = nullptr; int ld_dvt = 0; float beta_dvt = 0.f;
 };
 
@@ -538,11 +512,9 @@ struct Engine {
   float *x_init = nullptr, *x0 = nullptr, *chi_in = nullptr, *xi_in = nullptr, *frames = nullptr, *fbar = nullptr,
         *EE = nullptr, *XI = nullptr, *HP = nullptr;
   // backward state
-  float *DX = nullptr, *DHP = nullptr, *DH = nullptr, *DCHI = nullptr, *DMN = nullptr, *DFV = nullptr, *DME = nullptr,
-        *DMV = nullptr, *DS = nullptr, *DV = nullptr, *DPRE = nullptr, *DE = nullptr, *DXI = nullptr, *DEV = nullptr;
+  float *DX = nullptr, *DHP = nullptr, *DH = nullptr, *DCHI = nullptr, *DMN = nullptr, *DFV = nullptr, *DMV = nullptr,
+        *DS = nullptr, *DV = nullptr, *DPRE = nullptr, *DE = nullptr, *DXI = nullptr;
   Scratch sc{};
-  int variant = 0;              // 0: the straightforward graph; 1: split message GCP 0, activations on the tape, input
-                                // gradients written straight to their consumers (set before layout())
   float *PI = nullptr, *PJ = nullptr, *DVQ = nullptr;
   float* grad_base = nullptr;   // flat gradient buffer (reference layout), zeroed at the start of backward()
   size_t grad_count = 0;
@@ -579,8 +551,8 @@ struct Engine {
     g.z = take((size_t)M * S_out);
     g.up = V_out ? take((size_t)M * 3 * V_out) : nullptr;
     g.sg = V_out ? take((size_t)M * V_out) : nullptr;
-    g.a1t = (variant && V_out) ? take((size_t)M * S_out) : nullptr;
-    g.aff = (variant && ff) ? take((size_t)M * S_out) : nullptr;
+    g.a1t = V_out ? take((size_t)M * S_out) : nullptr;
+    g.aff = ff ? take((size_t)M * S_out) : nullptr;
   }
 
   // Lays out the tape for (dims, topology sizes).  Call with assign=false to size the arena, then with the arena.
@@ -602,7 +574,7 @@ struct Engine {
     for (int l = 0; l < d.L; ++l) {
       Layer& y = layers[l];
       const std::string p = "interaction_layers." + std::to_string(l) + ".";
-      shape_gcp(y.msg[0], p + "interaction.message_fusion.0.", E, 512 + d.Ed, 64 + d.Xd, 256, 32, 4, 0, 1, frames, look, variant);
+      shape_gcp(y.msg[0], p + "interaction.message_fusion.0.", E, 512 + d.Ed, 64 + d.Xd, 256, 32, 4, 0, 1, frames, look, 1);
       y.msg[0].vt = take((size_t)E * 3 * (64 + d.Xd)); y.msg[0].ldv = 64 + d.Xd;
       y.msg[0].Ed = d.Ed; y.msg[0].ee = EE; y.msg[0].rc = tp.edge_rc;
       for (int k = 0; k < 4; ++k) y.V[k] = take((size_t)E * 96);
@@ -622,14 +594,15 @@ struct Engine {
     shape_gcp(g_proj, "scalar_node_projection_gcp.", N, 256, 32, d.Hin, 0, 1, 0, 0, fbar, look);
     g_proj.vt = d.L ? layers[d.L - 1].CHI2 : nullptr; g_proj.ldv = 32;
     // scratch + backward state
-    sc.a1 = take((size_t)Mx * 256); sc.dz = take((size_t)Mx * 256); sc.dgz = take((size_t)Mx * 256);
+    sc.dz = take((size_t)Mx * 256); sc.dgz = take((size_t)Mx * 256);
     sc.dg = take((size_t)Mx * 32); sc.dup = take((size_t)Mx * 96); sc.dhid = take((size_t)Mx * 96); sc.dvdf = take((size_t)Mx * 9);
     sc.part = take((size_t)((Mx * 3 + kColsumRows - 1) / kColsumRows + 1) * 640);
     DX = take((size_t)N * 3); DHP = take((size_t)N * d.Hin); DH = take((size_t)N * 256); DCHI = take((size_t)N * 96);
-    DMN = take((size_t)N * 640); DFV = take((size_t)N * 3 * 64);
-    DME = take((size_t)E * (512 + d.Ed + (64 + d.Xd) / 4 + 9)); DMV = take((size_t)E * 3 * (64 + d.Xd));
+    // DMN: d s of the position GCP [N, 256], then d[agg_s | h] of the feed-forward GCP [N, 512]
+    DMN = take((size_t)N * 512); DFV = take((size_t)N * 3 * 64);
+    DMV = take((size_t)E * 3 * (64 + d.Xd));
     DS = take((size_t)E * 256); DV = take((size_t)E * 96); DPRE = take((size_t)E);
-    DE = take((size_t)E * d.Ed); DXI = take((size_t)E * 3 * d.Xd); DEV = take((size_t)E * 3);
+    DE = take((size_t)E * d.Ed); DXI = take((size_t)E * 3 * d.Xd);
     PI = take((size_t)N * 256); PJ = take((size_t)N * 256); DVQ = take((size_t)Mx * 48);
     for (int l = 0; l < d.L; ++l) { layers[l].msg[0].pi = PI; layers[l].msg[0].pj = PJ; }
     have_tape = false;
@@ -652,22 +625,20 @@ struct Engine {
     be.run(M * (g.H + 9), FMerge{g.hid, g.vdf, g.frames, g.merged, g.S_in, g.H, g.fan});
     const float* bias = g.bs;
     const float* Wm = g.Ws + g.wcol;      // the block of scalar_out's weight that multiplies `merged`
-    float* a1 = g.a1t ? g.a1t : sc.a1;
     if (g.ff) {
-      float* a = g.aff ? g.aff : sc.a1;
       be.gemm(false, true, M, g.S_out, g.fan, g.merged, g.fan, Wm, g.fanW, g.z1, g.S_out, 0.f);
-      be.run(M * g.S_out, FBiasSilu{g.z1, g.bs, a, g.S_out});
-      be.gemm(false, true, M, g.S_out, g.S_out, a, g.S_out, g.W2, g.S_out, g.z, g.S_out, 0.f);
+      be.run(M * g.S_out, FBiasSilu{g.z1, g.bs, g.aff, g.S_out});
+      be.gemm(false, true, M, g.S_out, g.S_out, g.aff, g.S_out, g.W2, g.S_out, g.z, g.S_out, 0.f);
       bias = g.b2;
     } else {
       be.gemm(false, true, M, g.S_out, g.fan, g.merged, g.fan, Wm, g.fanW, g.z, g.S_out, 0.f);
       if (g.split) be.gemm(false, true, M, g.S_out, g.Ed, g.ee, g.Ed, g.Ws + 256, g.fanW, g.z, g.S_out, 1.f);   // + e.We^T
     }
     be.run(M * g.S_out, FScalarOut{g.z, bias, g.S_out, g.act0, g.act1, s_out, ld_so, res_s, ld_rs, mask,
-                                   g.V_out ? a1 : nullptr, g.split ? g.pi : nullptr, g.pj, g.rc});
+                                   g.a1t, g.split ? g.pi : nullptr, g.pj, g.rc});
     if (!g.V_out) return;
     be.gemm(false, true, M * 3, g.V_out, g.H, g.hid, g.H, g.Wu, g.H, g.up, g.V_out, 0.f);           // vector_up
-    be.gemm(false, true, M, g.V_out, g.S_out, a1, g.S_out, g.Wg, g.S_out, g.sg, g.V_out, 0.f);      // vector_out_scale
+    be.gemm(false, true, M, g.V_out, g.S_out, g.a1t, g.S_out, g.Wg, g.S_out, g.sg, g.V_out, 0.f);   // vector_out_scale
     be.run(M * g.V_out, FVecOut{g.sg, g.bg, g.up, g.V_out, v_out, ld_vo, res_v, ld_rv, mask});
   }
 
@@ -680,9 +651,7 @@ struct Engine {
     const float* dgz = nullptr;
     if (g.V_out) {
       be.run(M * g.V_out, FDVecOut{dv_out, g.up, g.sg, ld_dv, g.V_out, sc.dg, sc.dup});
-      const float* a1 = g.a1t;
-      if (!a1) { be.run(M * g.S_out, FAct{g.z, sc.a1, g.act1}); a1 = sc.a1; }
-      be.gemm(true, false, g.V_out, g.S_out, M, sc.dg, g.V_out, a1, g.S_out, g.gWg, g.S_out, 1.f);
+      be.gemm(true, false, g.V_out, g.S_out, M, sc.dg, g.V_out, g.a1t, g.S_out, g.gWg, g.S_out, 1.f);
       colsum(sc.dg, M, g.V_out, g.V_out, g.gbg);
       be.gemm(false, false, M, g.S_out, g.V_out, sc.dg, g.V_out, g.Wg, g.S_out, sc.dgz, g.S_out, 0.f);
       be.gemm(true, false, g.V_out, g.H, M * 3, sc.dup, g.V_out, g.hid, g.H, g.gWu, g.H, 1.f);
@@ -692,9 +661,7 @@ struct Engine {
     be.run(M * g.S_out, FDZ{ds_out, ld_ds, dgz, g.z, g.S_out, g.act0, g.act1, sc.dz});
     const float* dzz = sc.dz;             // gradient at the output of the linear map that reads `merged`
     if (g.ff) {
-      const float* a = g.aff;
-      if (!a) { be.run(M * g.S_out, FAct{g.z1, sc.a1, 1}); a = sc.a1; }
-      be.gemm(true, false, g.S_out, g.S_out, M, sc.dz, g.S_out, a, g.S_out, g.gW2, g.S_out, 1.f);
+      be.gemm(true, false, g.S_out, g.S_out, M, sc.dz, g.S_out, g.aff, g.S_out, g.gW2, g.S_out, 1.f);
       colsum(sc.dz, M, g.S_out, g.S_out, g.gb2);
       be.gemm(false, false, M, g.S_out, g.S_out, sc.dz, g.S_out, g.W2, g.S_out, sc.dgz, g.S_out, 0.f);
       be.run(M * g.S_out, FMulDSilu{sc.dgz, g.z1});
@@ -702,31 +669,17 @@ struct Engine {
     }
     be.gemm(true, false, g.S_out, g.fan, M, dzz, g.S_out, g.merged, g.fan, g.gWs + g.wcol, g.fanW, 1.f);
     colsum(dzz, M, g.S_out, g.S_out, g.gbs);
-    const float* vq; int ldq, offq;
-    if (o.dvq) {
-      if (o.ds_dst && g.S_in)
-        be.gemm(false, false, M, g.S_in, g.S_out, dzz, g.S_out, g.Ws + g.wcol, g.fanW, o.ds_dst, o.ld_ds, o.beta_ds);
-      be.gemm(false, false, M, g.H + 9, g.S_out, dzz, g.S_out, g.Ws + g.wcol + g.S_in, g.fanW, o.dvq, g.H + 9, 0.f);
-      vq = o.dvq; ldq = g.H + 9; offq = 0;
-    } else {
-      be.gemm(false, false, M, g.fan, g.S_out, dzz, g.S_out, g.Ws + g.wcol, g.fanW, o.dmerged, g.fan, 0.f);
-      vq = o.dmerged; ldq = g.fan; offq = g.S_in;
-    }
-    be.run(M * g.H, FDNorm{vq, ldq, offq, g.H, g.hid, sc.dhid, g.V_out ? 1 : 0});
-    be.run(M * 9, FDQ{vq, ldq, offq + g.H, g.frames, sc.dvdf});
+    if (o.ds_dst && g.S_in)
+      be.gemm(false, false, M, g.S_in, g.S_out, dzz, g.S_out, g.Ws + g.wcol, g.fanW, o.ds_dst, o.ld_ds, o.beta_ds);
+    be.gemm(false, false, M, g.H + 9, g.S_out, dzz, g.S_out, g.Ws + g.wcol + g.S_in, g.fanW, DVQ, g.H + 9, 0.f);
+    be.run(M * g.H, FDNorm{DVQ, g.H + 9, g.H, g.hid, sc.dhid, g.V_out ? 1 : 0});
+    be.run(M * 9, FDQ{DVQ, g.H + 9, g.H, g.frames, sc.dvdf});
     be.gemm(true, false, 3, g.V_in, M * 3, sc.dvdf, 3, g.vt, g.ldv, g.gWf, g.V_in, 1.f);
     be.gemm(true, false, g.H, g.V_in, M * 3, sc.dhid, g.H, g.vt, g.ldv, g.gWd, g.V_in, 1.f);
     if (o.dvt) {
       be.gemm(false, false, M * 3, g.V_in, 3, sc.dvdf, 3, g.Wf, g.V_in, o.dvt, o.ld_dvt, o.beta_dvt);
       be.gemm(false, false, M * 3, g.V_in, g.H, sc.dhid, g.H, g.Wd, g.V_in, o.dvt, o.ld_dvt, 1.f);
     }
-  }
-  static BwdOut out0(float* dmerged, float* dvt, int ld_dvt, float beta_dvt) {
-    BwdOut o; o.dmerged = dmerged; o.dvt = dvt; o.ld_dvt = ld_dvt; o.beta_dvt = beta_dvt; return o;
-  }
-  BwdOut out1(float* ds_dst, int ld_ds, float beta_ds, float* dvt, int ld_dvt, float beta_dvt) {
-    BwdOut o; o.ds_dst = ds_dst; o.ld_ds = ld_ds; o.beta_ds = beta_ds; o.dvq = DVQ; o.dvt = dvt; o.ld_dvt = ld_dvt;
-    o.beta_dvt = beta_dvt; return o;
   }
 
   // ---------------------------------------------------------------------------------------------- network forward
@@ -749,12 +702,9 @@ struct Engine {
       const float* h = y.ff.merged + 256; const int ldh = y.ff.fan;      // this layer's input (h, chi) lives inside the
       const float* chi = y.FV + 32; const int ldc = 64;                   // feed-forward GCP's concatenated inputs
       Gcp& m0 = y.msg[0];
-      if (variant) {        // split form: the endpoint parts of scalar_out are node-level GEMMs, gathered in FScalarOut
-        be.gemm(false, true, N, 256, 256, h, ldh, m0.Ws, m0.fanW, PI, 256, 0.f);
-        be.gemm(false, true, N, 256, 256, h, ldh, m0.Ws + 256 + d.Ed, m0.fanW, PJ, 256, 0.f);
-      } else {
-        be.run(E * (512 + d.Ed), FGatherS{rc, h, ldh, EE, d.Ed, m0.merged, m0.fan});
-      }
+      // split form: the endpoint parts of scalar_out are node-level GEMMs, gathered in FScalarOut
+      be.gemm(false, true, N, 256, 256, h, ldh, m0.Ws, m0.fanW, PI, 256, 0.f);
+      be.gemm(false, true, N, 256, 256, h, ldh, m0.Ws + 256 + d.Ed, m0.fanW, PJ, 256, 0.f);
       be.run(E * 3 * (64 + d.Xd), FGatherV{rc, chi, ldc, XI, d.Xd, m0.vt});
       gcp_forward(m0, y.msg[1].merged, y.msg[1].fan, nullptr, 0, y.V[0], 32, nullptr, 0, nullptr);
       for (int k = 1; k < 4; ++k) {                                       // residual message GCPs (gcpnet.py:698-701)
@@ -790,71 +740,47 @@ struct Engine {
     const EdgeRc* rc = tp.edge_rc;
     if (grad_count) be.run((long long)grad_count, FFill{grad_base, 0.f});
     be.run(N, FDFinal{tp, d_out, d.F, d.Hin, DX, DHP});
-    if (variant) {
-      gcp_backward(g_proj, DHP, d.Hin, nullptr, 0, out1(DH, 256, 0.f, DCHI, 32, 0.f));
-    } else {
-      gcp_backward(g_proj, DHP, d.Hin, nullptr, 0, out0(DMN, DCHI, 32, 0.f));
-      be.run(N * 256, FCopy2D{DMN, g_proj.fan, DH, 256, 256});
-    }
+    gcp_backward(g_proj, DHP, d.Hin, nullptr, 0, BwdOut{DH, 256, 0.f, DCHI, 32, 0.f});
     if (E) { be.run(E * d.Ed, FFill{DE, 0.f}); be.run(E * 3 * d.Xd, FFill{DXI, 0.f}); }
     for (int l = d.L - 1; l >= 0; --l) {
       Layer& y = layers[l];
       Gcp& m0 = y.msg[0];
       const float* h = y.ff.merged + 256; const int ldh = y.ff.fan;
       // x_{l+1} = (x_l + pv) * mask and the frames are frozen: d x is the same masked vector at every layer
-      if (variant) {
-        gcp_backward(y.pos, nullptr, 0, DX, 1, out1(DMN, 256, 0.f, DFV, 32, 0.f));
-        be.run(N * 256, FMaskAdd{DH, 256, DMN, 256, 256, 1, tp.mask});
-      } else {
-        gcp_backward(y.pos, nullptr, 0, DX, 1, out0(DMN, DFV, 32, 0.f));
-        be.run(N * 256, FMaskAdd{DH, 256, DMN, y.pos.fan, 256, 1, tp.mask});
-      }
+      gcp_backward(y.pos, nullptr, 0, DX, 1, BwdOut{DMN, 256, 0.f, DFV, 32, 0.f});
+      be.run(N * 256, FMaskAdd{DH, 256, DMN, 256, 256, 1, tp.mask});
       be.run(N * 96, FMaskAdd{DCHI, 32, DFV, 32, 32, 3, tp.mask});
-      // feed-forward GCP: d[agg_s | h] -> DMN[:, :512] (row length ldm), d[agg_v | chi] -> DFV [N*3, 64]
-      const int ldm = variant ? 512 : y.ff.fan;
-      if (variant) gcp_backward(y.ff, DH, 256, DCHI, 32, out1(DMN, 512, 0.f, DFV, 64, 0.f));
-      else gcp_backward(y.ff, DH, 256, DCHI, 32, out0(DMN, DFV, 64, 0.f));
+      // feed-forward GCP: d[agg_s | h] -> DMN [N, 512], d[agg_v | chi] -> DFV [N*3, 64]
+      gcp_backward(y.ff, DH, 256, DCHI, 32, BwdOut{DMN, 512, 0.f, DFV, 64, 0.f});
       // message passing: d agg_s = DMN[:, :256], d agg_v = DFV[:, :32]
       if (E) {
-        be.run(E, FDAttnPre{rc, DMN, ldm, y.S3, y.attn, DPRE});
+        be.run(E, FDAttnPre{rc, DMN, 512, y.S3, y.attn, DPRE});
         be.gemm(true, false, 1, 256, E, DPRE, 1, y.S3, 256, y.gwa, 256, 1.f);
         colsum(DPRE, E, 1, 1, y.gba);
-        be.run(E * 256, FDAttnS{rc, DMN, ldm, y.attn, DPRE, y.wa, DS});
+        be.run(E * 256, FDAttnS{rc, DMN, 512, y.attn, DPRE, y.wa, DS});
         be.run(E * 96, FGatherRowV{rc, DFV, 64, DV});
-        for (int k = 3; k >= 1; --k) {
-          if (variant) {
-            gcp_backward(y.msg[k], DS, 256, DV, 32, out1(DS, 256, 1.f, DV, 32, 1.f));    // residual: += in place
-          } else {
-            gcp_backward(y.msg[k], DS, 256, DV, 32, out0(DME, DV, 32, 1.f));
-            be.run(E * 256, FAdd2D{DME, y.msg[k].fan, DS, 256, 256});
-          }
-        }
-        if (variant) gcp_backward(m0, DS, 256, DV, 32, out1(nullptr, 0, 0.f, DMV, 64 + d.Xd, 0.f));
-        else gcp_backward(m0, DS, 256, DV, 32, out0(DME, DMV, 64 + d.Xd, 0.f));
+        for (int k = 3; k >= 1; --k)
+          gcp_backward(y.msg[k], DS, 256, DV, 32, BwdOut{DS, 256, 1.f, DV, 32, 1.f});    // residual: += in place
+        gcp_backward(m0, DS, 256, DV, 32, BwdOut{nullptr, 0, 0.f, DMV, 64 + d.Xd, 0.f});
       }
-      be.run(N * 256, FAdd2D{DMN + 256, ldm, DH, 256, 256});
+      be.run(N * 256, FAdd2D{DMN + 256, 512, DH, 256, 256});
       be.run(N * 96, FAdd2D{DFV + 32, 64, DCHI, 32, 32});
       if (E) {
-        if (variant) {
-          // split message GCP 0: sc.dz is d z0 [E, 256].  e block of the weight, then the node-level endpoint blocks
-          be.gemm(true, false, 256, d.Ed, E, sc.dz, 256, EE, d.Ed, m0.gWs + 256, m0.fanW, 1.f);
-          be.gemm(false, false, E, d.Ed, 256, sc.dz, 256, m0.Ws + 256, m0.fanW, DE, d.Ed, 1.f);
-          be.run(N * 256, FScatterDZ{tp, apos, sc.dz, PI, PJ});        // PI / PJ reused as d PI / d PJ
-          be.gemm(true, false, 256, 256, N, PI, 256, h, ldh, m0.gWs, m0.fanW, 1.f);
-          be.gemm(true, false, 256, 256, N, PJ, 256, h, ldh, m0.gWs + 256 + d.Ed, m0.fanW, 1.f);
-          be.gemm(false, false, N, 256, 256, PI, 256, m0.Ws, m0.fanW, DH, 256, 1.f);
-          be.gemm(false, false, N, 256, 256, PJ, 256, m0.Ws + 256 + d.Ed, m0.fanW, DH, 256, 1.f);
-        } else {
-          be.run(N * 256, FScatterS{tp, apos, DME, m0.fan, d.Ed, DH, 256});
-          be.run(E * d.Ed, FAdd2D{DME + 256, m0.fan, DE, d.Ed, d.Ed});
-        }
+        // split message GCP 0: sc.dz is d z0 [E, 256].  e block of the weight, then the node-level endpoint blocks
+        be.gemm(true, false, 256, d.Ed, E, sc.dz, 256, EE, d.Ed, m0.gWs + 256, m0.fanW, 1.f);
+        be.gemm(false, false, E, d.Ed, 256, sc.dz, 256, m0.Ws + 256, m0.fanW, DE, d.Ed, 1.f);
+        be.run(N * 256, FScatterDZ{tp, apos, sc.dz, PI, PJ});        // PI / PJ reused as d PI / d PJ
+        be.gemm(true, false, 256, 256, N, PI, 256, h, ldh, m0.gWs, m0.fanW, 1.f);
+        be.gemm(true, false, 256, 256, N, PJ, 256, h, ldh, m0.gWs + 256 + d.Ed, m0.fanW, 1.f);
+        be.gemm(false, false, N, 256, 256, PI, 256, m0.Ws, m0.fanW, DH, 256, 1.f);
+        be.gemm(false, false, N, 256, 256, PJ, 256, m0.Ws + 256 + d.Ed, m0.fanW, DH, 256, 1.f);
         be.run(N * 96, FScatterV{tp, apos, DMV, 64 + d.Xd, d.Xd, DCHI, 32});
         be.run(E * 3 * d.Xd, FAdd2D{DMV + 32, 64 + d.Xd, DXI, d.Xd, d.Xd});
       }
     }
     // embedding inputs are data: no input gradient
-    gcp_backward(g_node, DH, 256, DCHI, 32, variant ? out1(nullptr, 0, 0.f, nullptr, 0, 0.f) : out0(DMN, nullptr, 0, 0.f));
-    gcp_backward(g_edge, DE, d.Ed, DXI, d.Xd, variant ? out1(nullptr, 0, 0.f, nullptr, 0, 0.f) : out0(DME, nullptr, 0, 0.f));
+    gcp_backward(g_node, DH, 256, DCHI, 32, BwdOut{});
+    gcp_backward(g_edge, DE, d.Ed, DXI, d.Xd, BwdOut{});
   }
 };
 

@@ -265,15 +265,10 @@ BDIFF_API int32_t bdiff_prepare_context(void* stream, const float* props, const 
  *   (the buffer is overwritten, not accumulated into).  No atomics: results are bit-reproducible.
  * bdiff_train_precision: tf32 = 0 (default) fp32 GEMMs, 1 = TF32 tensor-core GEMMs (the reference's bf16-mixed training
  *   configuration is the looser of the two).
- * bdiff_train_variant: 1 (default) = message GCP 0 in split form (node-level h.Wsi^T / h.Wsj^T instead of the [E, 512+Ed]
- *   gather + GEMM), activations kept on the tape and input gradients written straight into their consumers; 0 = the
- *   reference's operator graph one to one (same mathematics, 17 % slower; kept as the cross-check of variant 1).  Takes
- *   effect at the next bdiff_train_forward.
  * All on `stream`, no host synchronisation.  Errors: BDIFF_ESTATE without a plan / tape, BDIFF_ENOMEM for the tape. */
 BDIFF_API int64_t bdiff_param_floats(const bdiff_handle* h);
 BDIFF_API int32_t bdiff_param_layout(bdiff_handle* h, const char* name, int64_t* offset, int64_t* count);
 BDIFF_API int32_t bdiff_train_precision(bdiff_handle* h, int32_t tf32);
-BDIFF_API int32_t bdiff_train_variant(bdiff_handle* h, int32_t variant);
 /* Per-operation timing of the training pass: enable = 1 starts recording a CUDA event pair around every kernel and GEMM of
  * the following bdiff_train_forward / bdiff_train_backward calls (on their stream); enable = 0 synchronises `stream`, stops
  * and writes a table (operation, calls, total ms, share; sorted) into report[report_bytes] (NUL-terminated, truncated). */

@@ -47,7 +47,7 @@ extern "C" int hostcheck_train(const int* dims, int B, int N, long long E, int M
                                const int* act_idx, const long long* edge_off, const int* node_mol, const unsigned char* mask,
                                const int* edge_rc, const char* names, const long long* offsets, int nparams,
                                const float* params, float* grads, long long nfloats, const float* xh, const float* t,
-                               const float* ctx, const float* d_out, float* net_out, int variant) {
+                               const float* ctx, const float* d_out, float* net_out) {
   NetDims d{dims[0], dims[1], dims[2], dims[3], dims[4], dims[5]};
   Topo tp;
   tp.B = B; tp.N = N; tp.E = E; tp.Mact = Mact;
@@ -68,7 +68,6 @@ extern "C" int hostcheck_train(const int* dims, int B, int N, long long E, int M
   };
   HostBackend be;
   Engine<HostBackend> eng(be);
-  eng.variant = variant;
   const size_t need = eng.layout(d, tp, nullptr, look);
   if (missing) return -missing;
   std::vector<float> arena(need, 0.f);

@@ -89,14 +89,12 @@ def _autograd_case(cname, sizes, masked, seed=5):
     return cfg, bi, mask, xh, t, ctx, d_out
 
 
-@pytest.mark.parametrize("variant", [1, 0])
 @pytest.mark.parametrize("cname,sizes,masked", [("qm9", [19, 7, 12, 1, 25], [3, 30]), ("qm9_cond", [9, 14, 19], [0]),
                                                 ("geom", [44, 30, 3], [50])])
-def test_backward_matches_autograd_through_oracle(cname, sizes, masked, variant):
-    """Both engine variants (1 = default: split message GCP 0; 0 = the plain operator graph) against autograd."""
+def test_backward_matches_autograd_through_oracle(cname, sizes, masked):
+    """The training pass (forward and every parameter's gradient) against autograd through the oracle."""
     cfg, bi, mask, xh, t, ctx, d_out = _autograd_case(cname, sizes, masked)
     net, _, sd = make_net(cname, 21, scale=0.7)
-    net.set_train_variant(variant)
     sda = {k: v.clone().requires_grad_(True) for k, v in sd.items()}
     out_a = O.denoiser_forward(sda, cfg, bi, mask, xh, t, ctx)
     (out_a * d_out).sum().backward()

@@ -1,7 +1,6 @@
 """Where a training step spends its time: one CUDA event pair around every kernel and cuBLAS GEMM of the training pass
-(bdiff_train_timing), summed per operation, for one GEMM precision / engine variant.  Same batch as bench.py --config
-geom_train uses first (64 GEOM molecules, seed 1000).  Usage: python tools/train_step_profile.py [--tf32]  (env
-BDIFF_TRAIN_VARIANT selects the engine variant)."""
+(bdiff_train_timing), summed per operation, for one GEMM precision.  Same batch as bench.py --config geom_train uses
+first (64 GEOM molecules, seed 1000).  Usage: python tools/train_step_profile.py [--tf32]"""
 import ctypes as C
 import os
 import sys
@@ -57,7 +56,7 @@ def main():
     buf = C.create_string_buffer(1 << 16)
     _lib.check(h, lib.bdiff_train_timing(h, st, 0, buf, len(buf)), "bdiff_train_timing(off)")
     torch.cuda.synchronize()
-    print(f"# python tools/train_step_profile.py {' '.join(sys.argv[1:])}  BDIFF_TRAIN_VARIANT={os.environ.get('BDIFF_TRAIN_VARIANT', '0')}")
+    print(f"# python tools/train_step_profile.py {' '.join(sys.argv[1:])}")
     print(f"# one training step (loss forward + backward + optimiser), {B} GEOM molecules, {n} atoms, "
           f"{int((sizes.long() ** 2).sum())} edges: {ev0.elapsed_time(ev1):.2f} ms on the stream, events included")
     print(buf.value.decode())

@@ -95,7 +95,7 @@ __device__ __forceinline__ void run_seg(TcBars& B, uint32_t raddr, uint32_t& ci,
       wgmma_wait<0>();
       acc_fence<RS>(ts);
       acc_fence<RU>(tu);
-      if (lead) mbar_arrive(&B.empty[slot]);
+      mbar_arrive_if(&B.empty[slot], lead);
       ++ci;
       if (NS) {
 #pragma unroll
@@ -125,7 +125,9 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
   unsigned char* ring = smem + XE_BLOCKS * X_BLOCK;
   unsigned char* tail = ring + TC_NSLOT * TC_SLOT;
   TcBars& B = *reinterpret_cast<TcBars*>(tail);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // warp role and claimed item are broadcast with __shfl_sync so that ptxas can prove them warp-uniform: a wgmma on a
+  // path it cannot prove convergent serializes all of them (each waits for its own completion, ptxas C7520; see gemm)
+  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int hid0 = d.hid0;
   const int per_layer = q.TE + q.TN;
   const int total_items = q.nitems;                 // items of two tiles
@@ -215,14 +217,16 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
     // [128 + 32..63] node — one stamp before and after every GEMM phase, one at every accumulator read
     int es = 0;
     long long* stamp = nullptr;
-    auto PH = [&]() { if (stamp && tid == 0 && es < 32) stamp[es] = clock64(); ++es; };
+    auto PH = [&]() __attribute__((always_inline)) { if (stamp && tid == 0 && es < 32) stamp[es] = clock64(); ++es; };
     bool stamped[2] = {false, false};
     const uint32_t tl = (uint32_t)((warp & 3) * 32) << 16;       // this thread's scratch row quarter
     auto sz = [](int n) { return (uint32_t)((n * 4 + 15) & ~15); };
     for (uint32_t k = 0;; ++k) {
       const uint32_t slot = k & 1;
       mbar_wait(&B.item_full[slot], (k >> 1) & 1);
-      const int type = B.item[slot][0], layer = B.item[slot][1], tile = B.item[slot][2];
+      const int type = __shfl_sync(0xffffffffu, B.item[slot][0], 0);
+      const int layer = __shfl_sync(0xffffffffu, B.item[slot][1], 0);
+      const int tile = __shfl_sync(0xffffffffu, B.item[slot][2], 0);
       if (type < 0) break;
       if (tid == 0 && w.dbg && k < 16) {      // BDIFF_TIMING: {item code, t_fetch, t_start, t_end} for the first 16 items
         w.dbg[(size_t)blockIdx.x * 64 + 4 * k] = (type << 30) | (layer << 24) | tile;
@@ -304,9 +308,12 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
       PH();
       // GEMM phases run where the epilogue publishes an operand: both warpgroups issue their wgmmas and leave the
       // accumulators in the scratch, which the epilogue reads after the closing barrier.
+      // The lambdas are always inlined: compiled as a called subroutine, a GEMM phase is a path that ptxas cannot prove
+      // warp-uniform, and then it serializes EVERY wgmma of the kernel (C7520; tests/test_layers_sass.py).  Inlined, each
+      // publish site sees a constant phase, and a ring chunk's wgmmas issue back to back with one wait at its end.
       const int last = type == 1 && layer == q.L - 1;
       int ph = 0;
-      auto gemm = [&](int phase) {
+      auto gemm = [&](int phase) __attribute__((always_inline)) {
         if (type == 0) {
           const int ph = phase;
 #include "edge_tile_mma.inc"
@@ -315,10 +322,10 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
 #include "node_r4_tile_mma.inc"
         }
       };
-      auto publish = [&]() { fence_proxy_async(); named_bar_sync(3, TC_EPI); PH(); gemm(ph++); named_bar_sync(3, TC_EPI); PH(); };
-      auto wait_d = [&]() {};
+      auto publish = [&]() __attribute__((always_inline)) { fence_proxy_async(); named_bar_sync(3, TC_EPI); PH(); gemm(ph++); named_bar_sync(3, TC_EPI); PH(); };
+      auto wait_d = [&]() __attribute__((always_inline)) {};
       // node tile: U has been read (E3a), so G4 may overwrite its columns
-      auto release_u = [&]() { named_bar_sync(3, TC_EPI); gemm(-1); named_bar_sync(3, TC_EPI); };
+      auto release_u = [&]() __attribute__((always_inline)) { named_bar_sync(3, TC_EPI); gemm(-1); named_bar_sync(3, TC_EPI); };
       if (type == 0) {
         EdgeTail& T = *reinterpret_cast<EdgeTail*>(tail);
         const int half = tid >> 7, r = tid & 127;

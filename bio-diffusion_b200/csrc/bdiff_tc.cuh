@@ -87,6 +87,11 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive by the threads with `pred` set, as a predicated instruction rather than a branch (no divergent path between wgmmas)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %1, 0;\n@p mbarrier.arrive.shared::cta.b64 _, [%0];\n}\n" ::"r"(smem_u32(bar)),
+               "r"((int)pred) : "memory");
+}
 
 // ------------------------------------------------------------------------------------------ accumulator scratch
 // Base of this CTA's [512 columns][128 rows] fp32 scratch; set by the kernel before its first barrier.

@@ -19,6 +19,8 @@
 //
 // The TMA-producer lane also claims the tiles (so the next tile's weights stream while the current tile computes) and hands
 // them to the flag lane and the 8 compute warps through a two-slot mbarrier ring.
+#include <type_traits>
+
 #include "bdiff_node_tc.cuh"
 
 namespace bdiff {
@@ -54,12 +56,16 @@ constexpr int RING_CONSUMERS = TC_EPI / 32;       // one arrival per compute war
 // One weight-stream segment of a GEMM phase, run by both compute warpgroups (warpgroup wg: tile rows [64 wg, 64 wg + 64)).
 // For each N half h of the weight planes, `nch` ring chunks; issue(s, u, chunk address, c) issues the wgmmas of chunk c
 // into the accumulators s (NS columns, scratch columns scol + h NS) and u (NU columns at ucol + h NU), which start at
-// zero (fresh) or from the scratch.  Each chunk's products go into a fresh register tile that is then added to the running
-// sums with round-to-nearest fp32 adds: the tensor core's own fp32 accumulation truncates, and over a 1000-step chain
-// (where |h| grows by ~17 decades) that bias towards zero compounds into a visible drift from the fp32 path.
-template <int NS, int NU, class Issue>
+// zero (s: sfresh; u: bit h of ufresh) or from the scratch.  Each chunk's products go into a fresh register tile that is
+// then added to the running sums with round-to-nearest fp32 adds: the tensor core's own fp32 accumulation truncates, and
+// over a 1000-step chain (where |h| grows by ~17 decades) that bias towards zero compounds into a visible drift from the
+// fp32 path.  A finished half goes to the scratch, or, when an epilogue `epi(s, u, h, wg)` is given, to that functor
+// (fragment layout: frag_row / frag_col), which then runs between the halves' wgmmas: it must be always_inline and
+// free of divergent branches (see the kernel's note on C7520).
+struct AccToScratch {};
+template <int NS, int NU, class Issue, class Epi = AccToScratch>
 __device__ __forceinline__ void run_seg(TcBars& B, uint32_t raddr, uint32_t& ci, int nch, int scol, bool sfresh, int ucol,
-                                        bool ufresh, Issue&& issue) {
+                                        int ufresh, Issue&& issue, Epi&& epi = Epi{}) {
   constexpr int RS = NS ? NS / 2 : 1, RU = NU ? NU / 2 : 1;
   const int wg = threadIdx.x >> 7;
   const bool lead = (threadIdx.x & 31) == 0;
@@ -74,7 +80,7 @@ __device__ __forceinline__ void run_seg(TcBars& B, uint32_t raddr, uint32_t& ci,
       }
     }
     if (NU) {
-      if (ufresh) {
+      if ((ufresh >> h) & 1) {
 #pragma unroll
         for (int i = 0; i < RU; ++i) u[i] = 0.f;
       } else {
@@ -106,8 +112,12 @@ __device__ __forceinline__ void run_seg(TcBars& B, uint32_t raddr, uint32_t& ci,
         for (int i = 0; i < RU; ++i) u[i] += tu[i];
       }
     }
-    if (NS) acc_store<NS>(s, scol + h * NS, wg);
-    if (NU) acc_store<NU>(u, ucol + h * NU, wg);
+    if constexpr (std::is_same_v<std::decay_t<Epi>, AccToScratch>) {
+      if (NS) acc_store<NS>(s, scol + h * NS, wg);
+      if (NU) acc_store<NU>(u, ucol + h * NU, wg);
+    } else {
+      epi(s, u, h, wg);
+    }
   }
 }
 
@@ -307,7 +317,8 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
       if (w.dbg && k >= 2 && !stamped[type]) { stamp = w.dbg + 256 * 64 + (size_t)blockIdx.x * 64 + type * 32; stamped[type] = true; }
       PH();
       // GEMM phases run where the epilogue publishes an operand: both warpgroups issue their wgmmas and leave the
-      // accumulators in the scratch, which the epilogue reads after the closing barrier.
+      // accumulators in the scratch, which the epilogue reads after the closing barrier, or hand them to an elementwise
+      // epilogue in registers (edge tile: E0, E(k)b).
       // The lambdas are always inlined: compiled as a called subroutine, a GEMM phase is a path that ptxas cannot prove
       // warp-uniform, and then it serializes EVERY wgmma of the kernel (C7520; tests/test_layers_sass.py).  Inlined, each
       // publish site sees a constant phase, and a ring chunk's wgmmas issue back to back with one wait at its end.
@@ -322,7 +333,10 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
 #include "node_r4_tile_mma.inc"
         }
       };
-      auto publish = [&]() __attribute__((always_inline)) { fence_proxy_async(); named_bar_sync(3, TC_EPI); PH(); gemm(ph++); named_bar_sync(3, TC_EPI); PH(); };
+      // run: a GEMM phase whose epilogue runs inside it (writes the A tile, nothing to read back from the scratch), so the
+      // next publish follows directly; publish: a GEMM phase whose accumulators the epilogue reads after the barrier
+      auto run = [&]() __attribute__((always_inline)) { fence_proxy_async(); named_bar_sync(3, TC_EPI); PH(); gemm(ph++); };
+      auto publish = [&]() __attribute__((always_inline)) { run(); named_bar_sync(3, TC_EPI); PH(); };
       auto wait_d = [&]() __attribute__((always_inline)) {};
       // node tile: U has been read (E3a), so G4 may overwrite its columns
       auto release_u = [&]() __attribute__((always_inline)) { named_bar_sync(3, TC_EPI); gemm(-1); named_bar_sync(3, TC_EPI); };
@@ -338,6 +352,7 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
         const int l = lane, s = warp, c0 = warp * 32;
         const SmallWR4& sw = T.sw;
         (void)T;
+        (void)run;
 #include "node_r4_tile_epilogue.inc"
       }
       PH();

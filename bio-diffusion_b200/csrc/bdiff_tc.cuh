@@ -8,6 +8,7 @@
 //   B: un-swizzled K=16 slabs (see bdiff_slab.cuh), descriptor with explicit LBO / SBO.
 //   Accumulators: registers of the issuing warpgroup, stored at the end of a GEMM phase to a per-CTA scratch of 128 rows
 //   x 512 columns (column-major) that the epilogue threads read by row; scratch addresses are (row << 16) | column.
+//   Elementwise epilogues instead run on the registers themselves (frag_row / frag_col give each register's place).
 #pragma once
 #include <cuda_bf16.h>
 #include <stdint.h>
@@ -99,20 +100,25 @@ __shared__ float* tm_base;
 __device__ __forceinline__ float* tm_word(uint32_t taddr) {
   return tm_base + (size_t)(taddr & 0xffffu) * 128 + (taddr >> 16) + (threadIdx.x & 31);
 }
-// wgmma fragment of an M=64 x N tile (rows 64 wg .. 64 wg + 63 of the scratch, columns col0 ..) <-> scratch
+// wgmma fragment of an M=64 x N tile issued by warpgroup wg: register j of this thread holds the element at row
+// frag_row(wg, j) of the 128-row tile and column frag_col(j) of the tile's N columns.  Registers j and j + 1 (j even)
+// are two adjacent columns of one row.
+__device__ __forceinline__ int frag_row(int wg, int j) {
+  return 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((j >> 1) & 1);
+}
+__device__ __forceinline__ int frag_col(int j) { return 8 * (j >> 2) + 2 * (threadIdx.x & 3) + (j & 1); }
+// fragment (columns col0 ..) <-> scratch
 template <int N>
 __device__ __forceinline__ void acc_store(const float* d, int col0, int wg) {
-  const int lane = threadIdx.x & 31, row = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+  float* const base = tm_base;     // one read of the pointer (a store through float* could alias it)
 #pragma unroll
-  for (int j = 0; j < N / 2; ++j)
-    tm_base[(size_t)(col0 + 8 * (j >> 2) + 2 * (lane & 3) + (j & 1)) * 128 + row + 8 * ((j >> 1) & 1)] = d[j];
+  for (int j = 0; j < N / 2; ++j) base[(size_t)(col0 + frag_col(j)) * 128 + frag_row(wg, j)] = d[j];
 }
 template <int N>
 __device__ __forceinline__ void acc_load(float* d, int col0, int wg) {
-  const int lane = threadIdx.x & 31, row = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+  const float* const base = tm_base;
 #pragma unroll
-  for (int j = 0; j < N / 2; ++j)
-    d[j] = tm_base[(size_t)(col0 + 8 * (j >> 2) + 2 * (lane & 3) + (j & 1)) * 128 + row + 8 * ((j >> 1) & 1)];
+  for (int j = 0; j < N / 2; ++j) d[j] = base[(size_t)(col0 + frag_col(j)) * 128 + frag_row(wg, j)];
 }
 
 // scratch -> registers: this thread's row (32*(warp%4) + laneid, encoded in taddr's upper half), `N` consecutive columns

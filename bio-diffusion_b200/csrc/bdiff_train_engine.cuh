@@ -90,10 +90,10 @@ struct FCentre {        // x = x_init - mask * mean_mol(x_init)                 
       s0 += x_init[j * 3 + 0]; s1 += x_init[j * 3 + 1]; s2 += x_init[j * 3 + 2];
       cnt += tp.mask[j] ? 1.0f : 0.0f;
     }
-    const float m = tp.mask[i] ? 1.0f : 0.0f;
-    x[i * 3 + 0] = x_init[i * 3 + 0] - (s0 / cnt) * m;
-    x[i * 3 + 1] = x_init[i * 3 + 1] - (s1 / cnt) * m;
-    x[i * 3 + 2] = x_init[i * 3 + 2] - (s2 / cnt) * m;
+    const float m = tp.mask[i] ? 1.0f : 0.0f;     // a molecule without active atoms has the centroid 0 (DESIGN.md §2)
+    x[i * 3 + 0] = x_init[i * 3 + 0] - (cnt > 0.f ? s0 / cnt : 0.f) * m;
+    x[i * 3 + 1] = x_init[i * 3 + 1] - (cnt > 0.f ? s1 / cnt : 0.f) * m;
+    x[i * 3 + 2] = x_init[i * 3 + 2] - (cnt > 0.f ? s2 / cnt : 0.f) * m;
   }
 };
 struct FOrient {        // chi_in over the concatenated atom list                      (protein_graph_dataset.py:217-225)
@@ -426,7 +426,7 @@ struct FFinal {         // net_out = [centralize((x_L - x_init) * mask) | hp[:, 
     }
     const float m = tp.mask[i] ? 1.0f : 0.0f;
     float* o = out + i * (3 + F);
-    for (int x = 0; x < 3; ++x) o[x] = (xL[i * 3 + x] - x_init[i * 3 + x]) * m - (s[x] / cnt) * m;
+    for (int x = 0; x < 3; ++x) o[x] = (xL[i * 3 + x] - x_init[i * 3 + x]) * m - (cnt > 0.f ? s[x] / cnt : 0.f) * m;
     for (int j = 0; j < F; ++j) o[3 + j] = hp[i * ld_hp + j];
   }
 };
@@ -441,7 +441,7 @@ struct FDFinal {        // d x_L and d hp from d net_out
       cnt += m;
     }
     const float m = tp.mask[i] ? 1.0f : 0.0f;
-    for (int x = 0; x < 3; ++x) dx[i * 3 + x] = (dout[i * (3 + F) + x] - s[x] / cnt) * m;
+    for (int x = 0; x < 3; ++x) dx[i * 3 + x] = (dout[i * (3 + F) + x] - (cnt > 0.f ? s[x] / cnt : 0.f)) * m;
     for (int j = 0; j < Hin; ++j) dhp[i * Hin + j] = j < F ? dout[i * (3 + F) + 3 + j] : 0.0f;
   }
 };

@@ -132,13 +132,16 @@ def edge_features(x: torch.Tensor, ei: torch.Tensor) -> Tuple[torch.Tensor, torc
 
 
 def centralize(x: torch.Tensor, batch_index: torch.Tensor, mask: torch.Tensor,
-               num_mols: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """x - mask * (sum_mol x / sum_mol mask)   (components/__init__.py:46-98, edm=True branch)."""
+               num_mols: Optional[int] = None, guard_empty: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x - mask * (sum_mol x / sum_mol mask)   (components/__init__.py:46-98, edm=True branch).
+
+    A molecule without active atoms has the centroid 0/0 = NaN, as in the reference; guard_empty=True makes it 0
+    instead (what the CUDA path computes, DESIGN.md §2)."""
     b = int(batch_index.max().item()) + 1 if num_mols is None else num_mols
     mf = mask.to(x.dtype)
     cnt = torch.zeros(b, dtype=x.dtype).index_add_(0, batch_index, mf)
     tot = torch.zeros((b, x.shape[1]), dtype=x.dtype).index_add_(0, batch_index, x)
-    cen = tot / cnt.unsqueeze(-1)
+    cen = tot / (cnt.clamp(min=1) if guard_empty else cnt).unsqueeze(-1)
     return cen, x - cen[batch_index] * mf.unsqueeze(-1)
 
 
@@ -227,7 +230,7 @@ def message_passing(sd, p: str, cfg: OracleConfig, h, chi, e, xi, ei, frames, ta
     s = s * attn
     if taps is not None:
         taps["msg_s"], taps["msg_v"] = s, v
-    flat = torch.cat((s, v.reshape(v.shape[0], -1)), dim=-1)   # ScalarVector.flatten (:713)
+    flat = torch.cat((s, v.flatten(1)), dim=-1)                # ScalarVector.flatten (:713)
     agg = torch.zeros((h.shape[0], flat.shape[1]), dtype=flat.dtype).index_add_(0, r, flat)   # (:723)
     vd = cfg.chi_hidden
     return agg[:, :-3 * vd], agg[:, -3 * vd:].reshape(-1, vd, 3)
@@ -252,8 +255,11 @@ def interaction_layer(sd, p: str, cfg: OracleConfig, h, chi, e, xi, ei, frames, 
 def denoiser_forward(sd: Dict[str, torch.Tensor], cfg: OracleConfig, batch_index: torch.Tensor,
                      mask: torch.Tensor, xh: torch.Tensor, t: torch.Tensor,
                      context: Optional[torch.Tensor] = None, taps: Optional[dict] = None,
-                     dtype=torch.float32) -> torch.Tensor:
-    """GCPNetDynamics.atom_types_and_coords_forward (gcpnet.py:1069-1232) -> net_out [N, 3+F]."""
+                     dtype=torch.float32, guard_empty: bool = False) -> torch.Tensor:
+    """GCPNetDynamics.atom_types_and_coords_forward (gcpnet.py:1069-1232) -> net_out [N, 3+F].
+
+    guard_empty: see `centralize`.  Without it, a molecule with no active atoms gets NaN coordinate rows, and the NaN guard
+    below then zeroes the velocity of every molecule in the batch (the reference's behaviour)."""
     sd = {k: v.to(dtype) for k, v in sd.items()}
     mask_f = mask.to(dtype)
     xh = xh.to(dtype) * mask_f[:, None]                        # (:1081)
@@ -265,7 +271,7 @@ def denoiser_forward(sd: Dict[str, torch.Tensor], cfg: OracleConfig, batch_index
     if cfg.num_context:
         h_in = torch.cat((h_in, context.to(dtype).reshape(xh.shape[0], cfg.num_context)), dim=-1)
     nmol = int(batch_index.max().item()) + 1
-    _, x = centralize(x_init, batch_index, mask, nmol)         # (:1160-1166)
+    _, x = centralize(x_init, batch_index, mask, nmol, guard_empty)     # (:1160-1166)
     frames = localize(x, ei)                                   # (:1169-1174) frozen across layers
     # embedding (gcpnet.py:551-603): edge GCP2 silu/silu, node GCP2 no activation
     e, xi = gcp2(sd, "gcp_embedding.edge_embedding.", e_in, xi_in, ei, frames, False, ("silu", "silu"))
@@ -286,7 +292,7 @@ def denoiser_forward(sd: Dict[str, torch.Tensor], cfg: OracleConfig, batch_index
     h_final = hp[:, :cfg.num_h]                                # (:1208-1211) strip ctx + time
     if torch.isnan(vel).any():                                 # (:1214-1216)
         vel = torch.zeros_like(vel)
-    _, vel = centralize(vel, batch_index, mask, nmol)          # (:1219-1227)
+    _, vel = centralize(vel, batch_index, mask, nmol, guard_empty)      # (:1219-1227)
     return torch.cat((vel, h_final), dim=-1)                   # (:1230)
 
 

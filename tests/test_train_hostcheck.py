@@ -82,7 +82,8 @@ def run_hostcheck(lib, cfg, sd, bi, mask, xh, t, ctx, d_out):
 
 
 @pytest.mark.parametrize("cname,sizes,masked", [("qm9", [5, 1, 7], [2]), ("qm9_cond", [4, 6], [5]), ("geom", [9, 3, 1], [0, 10]),
-                                                ("geom", [4, 4], []), ("geom", [131, 2], [7])])
+                                                ("geom", [4, 4], []), ("geom", [131, 2], [7]),
+                                                ("qm9", [3, 4, 5], [3, 4, 5, 6])])      # molecule 1 has no active atom
 def test_training_pass_matches_autograd(cname, sizes, masked):
     lib = build_hostcheck()
     cfg = O.config_named(cname)
@@ -99,7 +100,7 @@ def test_training_pass_matches_autograd(cname, sizes, masked):
     ctx = torch.randn((n, cfg.num_context), generator=g) if cfg.num_context else None
     d_out = torch.randn((n, 3 + cfg.num_h), generator=g)
     sda = {k: v.clone().requires_grad_(True) for k, v in sd.items()}
-    out_a = O.denoiser_forward(sda, cfg, bi, mask, xh, t, ctx)
+    out_a = O.denoiser_forward(sda, cfg, bi, mask, xh, t, ctx, guard_empty=True)    # DESIGN.md §2
     (out_a * d_out).sum().backward()
     out_h, grads = run_hostcheck(lib, cfg, sd, bi, mask, xh, t, ctx, d_out)
     err_f = (out_h - out_a.detach()).abs().max().item() / out_a.detach().abs().max().item()

@@ -387,7 +387,7 @@ int32_t bdiff_selftest_split(void* stream, int32_t variant, const float* A, cons
   if (selftest_configure() != cudaSuccess) return BDIFF_ECUDA;
   void* img = nullptr;
   if (cudaMalloc(&img, selftest_img_bytes()) != cudaSuccess) return BDIFF_ENOMEM;
-  launch_umma_selftest_split(st, A, W, static_cast<unsigned char*>(img), C, variant);
+  launch_wgmma_selftest_split(st, A, W, static_cast<unsigned char*>(img), C, variant);
   cudaError_t e = cudaStreamSynchronize(st);
   cudaFree(img);
   return e == cudaSuccess ? BDIFF_OK : BDIFF_ECUDA;

@@ -7,21 +7,55 @@
 namespace bdiff {
 
 constexpr int TMT = 128;                 // edges per tile
-// weight ring: TC_NSLOT slots of TC_SLOT bytes; a chunk is one K step of one N half of a weight plane (hi plane + lo
-// plane, N/2 rows x 32 B each) or a group of small K steps, always a single contiguous TMA bulk copy
-constexpr int TC_SLOT = 2 * 160 * 32;    // 10 KiB: one N half of the widest K step
+// weight ring: TC_NSLOT slots of TC_SLOT bytes; a chunk is always a single contiguous TMA bulk copy
+constexpr int TC_SLOT = 2 * 160 * 32;    // 10 KiB: one N half of the widest K step (checked against the stream tables)
 constexpr int TC_NSLOT = 5;
 // accumulator-scratch column map of an edge tile (512 columns)
 constexpr int TM_S = 0, TM_U0 = 256, TM_U1 = 288, TM_MV = 320, TM_VD0 = 416;
 constexpr int TM_EX = 416, TM_EX_STRIDE = 40;     // pair-exchange scratch (over VD0, which is dead by then): 2 x 40 columns
 
-__host__ __device__ inline int tc_k0_steps(int Ed, int Xd) {     // K=16 steps of message GCP 0's edge part
+// ---- The weight stream of one (pass, layer), defined here and nowhere else: the pack kernels (bdiff_tc_pack.cu), the
+// TMA lane and the GEMM phases of the megakernel all walk these tables.
+// A stream is [N half 0 | N half 1]: every weight plane is split in two, and the megakernel multiplies one half at a
+// time.  A half is a sequence of segments.  A segment is `steps` K=16 steps; a step is [hi plane | lo plane] of `rows`
+// local rows each (slab layout of bdiff_slab.cuh, 2 * rows * 32 bytes).  `group` steps travel as one ring chunk (the
+// last chunk of a segment may be short).  The consumer takes all chunks of a segment for half 0, then for half 1.
+// The 2 * rows plane rows of a step are, in order: [128 product rows of half 0 | of half 1 | gate rows of half 0 | of
+// half 1] (planes of fewer than 128 rows have no gate rows); a half's local rows are its product rows, then its gate rows.
+struct StreamSeg { int steps, rows, group; };
+struct Stream { StreamSeg seg[8]; int n; };
+__host__ __device__ constexpr int seg_step_bytes(StreamSeg g) { return 2 * g.rows * 32; }
+__host__ __device__ constexpr int seg_chunks(StreamSeg g) { return (g.steps + g.group - 1) / g.group; }
+__host__ __device__ constexpr size_t stream_bytes(const Stream& s) {        // both halves
+  size_t b = 0;
+  for (int i = 0; i < s.n; ++i) b += (size_t)s.seg[i].steps * 2 * seg_step_bytes(s.seg[i]);
+  return b;
+}
+__host__ __device__ constexpr long long stream_plane_rows(const Stream& s) {      // plane rows of both halves, all steps
+  long long r = 0;
+  for (int i = 0; i < s.n; ++i) r += (long long)s.seg[i].steps * 2 * s.seg[i].rows;
+  return r;
+}
+__host__ __device__ constexpr int stream_max_chunk(const Stream& s) {
+  int m = 0;
+  for (int i = 0; i < s.n; ++i) {
+    const int c = s.seg[i].group * seg_step_bytes(s.seg[i]);
+    m = c > m ? c : m;
+  }
+  return m;
+}
+
+__host__ __device__ constexpr int tc_k0_steps(int Ed, int Xd) {     // K=16 steps of message GCP 0's edge part
   return (Ed + (64 + Xd) / 4 + 9 + 15) / 16;
 }
-// bytes of one layer's edge-pass weight stream (see k_pack_edge_slabs for the order)
-__host__ __device__ inline size_t tc_edge_stream_bytes(int Ed, int Xd) {
-  return (size_t)tc_k0_steps(Ed, Xd) * 2 * 256 * 32 + 3 * ((size_t)16 * 2 * 320 * 32 + 2 * 2 * 256 * 32) + (size_t)16 * 2 * 32 * 32;
+// Edge pass: entry i is GEMM phase i of edge_tile_mma.inc.
+//   G0: W0e, zero-padded to k0s * 16 K rows;  G(k)a, k = 1..3: [W_k rows | 32 gate rows: half 0 -> U0, half 1 -> U1];
+//   G(k)b: W_k K rows 256..287;  G4: Wg_3, four K steps per chunk.
+__host__ __device__ constexpr Stream tc_edge_stream(int k0s) {
+  constexpr StreamSeg Ga{16, 160, 1}, Gb{2, 128, 1};
+  return {{{k0s, 128, 1}, Ga, Gb, Ga, Gb, Ga, Gb, {16, 16, 4}}, 8};
 }
+static_assert(stream_max_chunk(tc_edge_stream(8)) <= TC_SLOT, "an edge-pass chunk must fit a ring slot");
 
 // mbarriers / bookkeeping of the megakernel; first member (base class) of both tile tails
 struct TcBars {
@@ -62,7 +96,7 @@ struct EdgeTail : TcBars {
 // and this thread's partial vector_down / vector_down_frames sums of the NEXT GCP.
 // HP = hidden dim of the previous GCP; vdp = its vector_down output (full, [HP][3]).
 template <int HP, bool FIRST, bool LAST>
-__device__ __forceinline__ void gate_update(uint32_t tl, int half, int ucol, const float* __restrict__ vdp,
+__device__ __forceinline__ void gate_update(int half, int ucol, const float* __restrict__ vdp,
                                             const float* __restrict__ Wu, const float* __restrict__ bgp,
                                             const float* __restrict__ Wdn, const float* __restrict__ Wfn,
                                             float* __restrict__ part) {   // part[33]: partial VD_next(24)+VDF_next(9)
@@ -75,22 +109,8 @@ __device__ __forceinline__ void gate_update(uint32_t tl, int half, int ucol, con
   }
   for (int oc = half * 2; oc < half * 2 + 2; ++oc) {
     float u[8], mv[24];
-    {
-      uint32_t ru[8], rm[24];
-      tmem_ld8_nw(tl + ucol + oc * 8, ru);
-      if (!FIRST) {
-        tmem_ld8_nw(tl + TM_MV + oc * 24, rm);
-        tmem_ld8_nw(tl + TM_MV + oc * 24 + 8, rm + 8);
-        tmem_ld8_nw(tl + TM_MV + oc * 24 + 16, rm + 16);
-      }
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 8; ++i) u[i] = __uint_as_float(ru[i]);
-      if (!FIRST) {
-#pragma unroll
-        for (int i = 0; i < 24; ++i) mv[i] = __uint_as_float(rm[i]);
-      }
-    }
+    scratch_ld<8>(ucol + oc * 8, u);
+    if (!FIRST) scratch_ld<24>(TM_MV + oc * 24, mv);
 #pragma unroll
     for (int jp = 0; jp < 4; ++jp) {          // two output channels (j = 2jp, 2jp+1) per packed instruction
       const int o = oc * 8 + 2 * jp;
@@ -114,7 +134,7 @@ __device__ __forceinline__ void gate_update(uint32_t tl, int half, int ucol, con
       }
       mv[ja + 0] = r0.x; mv[jb + 0] = r0.y; mv[ja + 1] = r1.x; mv[jb + 1] = r1.y; mv[ja + 2] = r2.x; mv[jb + 2] = r2.y;
     }
-    tmem_st8xN<3>(tl + TM_MV + oc * 24, mv);      // completion awaited once, at the end of the function
+    scratch_st<24>(TM_MV + oc * 24, mv);
     if (!LAST) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -144,24 +164,20 @@ __device__ __forceinline__ void gate_update(uint32_t tl, int half, int ucol, con
 #pragma unroll
       for (int x = 0; x < 3; ++x) { part[(2 * hp) * 3 + x] = p2[hp][x].x; part[(2 * hp + 1) * 3 + x] = p2[hp][x].y; }
   }
-  tmem_st_wait();
 }
 
 // The two threads of a pair (same scratch row) swap their 33 partial sums through scratch columns.
 // Callers guarantee that nobody still reads the columns (VD0) being overwritten.
-__device__ __forceinline__ void pair_exchange33(uint32_t tl, int half, const float* __restrict__ mine, float* __restrict__ theirs) {
+__device__ __forceinline__ void pair_exchange33(int half, const float* __restrict__ mine, float* __restrict__ theirs) {
   float pad[40];
 #pragma unroll
   for (int i = 0; i < 33; ++i) pad[i] = mine[i];
 #pragma unroll
   for (int i = 33; i < 40; ++i) pad[i] = 0.f;
-  tmem_st8xN<5>(tl + TM_EX + half * TM_EX_STRIDE, pad);
-  tmem_st_wait();
-  tc_fence_before();
+  scratch_st<40>(TM_EX + half * TM_EX_STRIDE, pad);
   named_bar_sync(3, TC_EPI);
-  tc_fence_after();
   float got[40];
-  tmem_ld8xN<5>(tl + TM_EX + (half ^ 1) * TM_EX_STRIDE, got);
+  scratch_ld<40>(TM_EX + (half ^ 1) * TM_EX_STRIDE, got);
 #pragma unroll
   for (int i = 0; i < 33; ++i) theirs[i] = got[i];
 }

@@ -90,7 +90,7 @@ void launch_layers_tc(cudaStream_t st, const Plan& p, const Dims& d, const Embed
                       const Work& w, int num_sms);
 cudaError_t selftest_configure();
 size_t selftest_img_bytes();
-void launch_umma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
+void launch_wgmma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
                                 int variant);
 
 }  // namespace bdiff

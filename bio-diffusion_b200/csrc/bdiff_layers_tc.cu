@@ -54,7 +54,7 @@ static_assert(256 * LAYERS_REG_COMPUTE + 128 * LAYERS_REG_SERVICE <= 168 * LAYER
 constexpr int RING_CONSUMERS = TC_EPI / 32;       // one arrival per compute warp frees a ring slot
 
 // One weight-stream segment of a GEMM phase, run by both compute warpgroups (warpgroup wg: tile rows [64 wg, 64 wg + 64)).
-// For each N half h of the weight planes, `nch` ring chunks; issue(s, u, chunk address, c) issues the wgmmas of chunk c
+// For each N half h of the weight planes, `nch` = seg_chunks(stream-table entry) ring chunks; issue(s, u, chunk address, c) issues the wgmmas of chunk c
 // into the accumulators s (NS columns, scratch columns scol + h NS) and u (NU columns at ucol + h NU), which start at
 // zero (s: sfresh; u: bit h of ufresh) or from the scratch.  Each chunk's products go into a fresh register tile that is
 // then added to the running sums with round-to-nearest fp32 adds: the tensor core's own fp32 accumulation truncates, and
@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
     mbar_init(&B.tile_done, TC_EPI);
     mbar_init(&B.wbar, 1);
     mbar_fence_init();
-    tm_base = w.acc + (size_t)blockIdx.x * TM_COLS * 128;
+    acc_scratch = w.acc + (size_t)blockIdx.x * TM_COLS * 128;
   }
   __syncthreads();
 
@@ -173,27 +173,24 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
         B.item[slot][0] = type; B.item[slot][1] = layer; B.item[slot][2] = tile;
         mbar_arrive(&B.item_full[slot]);
         if (type < 0) break;
-        // the layer's weight stream: [N half 0 stream | N half 1 stream]; each segment streams half 0, then half 1
+        // the layer's weight stream (tc_edge_stream / tc_node_stream): per segment, the chunks of N half 0, then of half 1
         const size_t stride = type == 0 ? q.edge_blob_stride : q.node_blob_stride;
         const unsigned char* blob = (type == 0 ? q.edge_blob : q.node_blob) + (size_t)layer * stride;
+        const Stream S = type == 0 ? tc_edge_stream(K0S) : tc_node_stream(layer == q.L - 1);
         size_t off = 0;
-        auto push_half = [&](int h, size_t rel, uint32_t bytes) {
-          const uint32_t s = ci % TC_NSLOT;
-          mbar_wait_backoff(&B.empty[s], ((ci / TC_NSLOT) & 1) ^ 1);
-          mbar_expect_tx(&B.full[s], bytes);
-          bulk_g2s(ring + s * TC_SLOT, blob + h * (stride / 2) + off + rel, bytes, &B.full[s]);
-          ++ci;
-        };
-        auto seg = [&](int n, uint32_t bytes) {
+        for (int i = 0; i < S.n; ++i) {
+          const StreamSeg g = S.seg[i];
+          const uint32_t step = seg_step_bytes(g);
           for (int h = 0; h < 2; ++h)
-            for (int c = 0; c < n; ++c) push_half(h, (size_t)c * bytes, bytes);
-          off += (size_t)n * bytes;
-        };
-        if (type == 0) {
-#include "edge_tile_producer.inc"
-        } else {
-          const int last = layer == q.L - 1;
-#include "node_r4_tile_producer.inc"
+            for (int c = 0; c < seg_chunks(g); ++c) {
+              const int steps = min(g.group, g.steps - c * g.group);
+              const uint32_t s = ci % TC_NSLOT;
+              mbar_wait_backoff(&B.empty[s], ((ci / TC_NSLOT) & 1) ^ 1);
+              mbar_expect_tx(&B.full[s], steps * step);
+              bulk_g2s(ring + s * TC_SLOT, blob + h * (stride / 2) + off + (size_t)c * g.group * step, steps * step, &B.full[s]);
+              ++ci;
+            }
+          off += (size_t)g.steps * step;
         }
       }
     }
@@ -229,7 +226,6 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
     long long* stamp = nullptr;
     auto PH = [&]() __attribute__((always_inline)) { if (stamp && tid == 0 && es < 32) stamp[es] = clock64(); ++es; };
     bool stamped[2] = {false, false};
-    const uint32_t tl = (uint32_t)((warp & 3) * 32) << 16;       // this thread's scratch row quarter
     auto sz = [](int n) { return (uint32_t)((n * 4 + 15) & ~15); };
     for (uint32_t k = 0;; ++k) {
       const uint32_t slot = k & 1;
@@ -247,36 +243,40 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
         named_bar_sync(3, TC_EPI);             // everybody is done with the previous set
         if (tid == 0) {
           const LayerW lw = q.layers[layer];       // by value: the pointer loads go out together, not one per copy
+          // every (destination, source, count) is listed once and visited twice: for the byte total, then for the copies
+          auto stage = [&](auto&& list) {
+            uint32_t total = 0;
+            list([&](float*, const float*, int n) { total += sz(n); });
+            mbar_expect_tx(&B.wbar, total);
+            list([&](float* dst, const float* src, int n) { bulk_g2s(dst, src, sz(n), &B.wbar); });
+          };
           if (type == 0) {
             SmallW& s = reinterpret_cast<EdgeTail*>(tail)->sw;
-            mbar_expect_tx(&B.wbar, sz(XD * HID0) + sz(XD * 3) + sz(HID0 * 32) +
-                                        3 * (sz(256) + sz(256) + sz(256) + sz(96) + sz(32)) + sz(32) + sz(256) + sz(1));
-            auto cp = [&](float* dst, const float* src, int n) { bulk_g2s(dst, src, sz(n), &B.wbar); };
-            cp(s.Wd0x, lw.Wd0x, XD * HID0); cp(s.Wf0x, lw.Wf0x, XD * 3); cp(s.Wu0, lw.Wu0, HID0 * 32);
-            for (int kk = 0; kk < 3; ++kk) {
-              cp(s.Wdk[kk], lw.Wdk[kk], 256); cp(s.Wuk[kk], lw.Wuk[kk], 256); cp(s.bk[kk], lw.bk[kk], 256);
-              cp(s.Wfk[kk], lw.Wfk[kk], 96); cp(s.bg[kk + 1], lw.bgk[kk], 32);
-            }
-            cp(s.bg[0], lw.bg0, 32); cp(s.wa, lw.wa, 256); cp(s.ba, lw.ba, 1);
+            stage([&](auto&& cp) {
+              cp(s.Wd0x, lw.Wd0x, XD * HID0); cp(s.Wf0x, lw.Wf0x, XD * 3); cp(s.Wu0, lw.Wu0, HID0 * 32);
+              for (int kk = 0; kk < 3; ++kk) {
+                cp(s.Wdk[kk], lw.Wdk[kk], 256); cp(s.Wuk[kk], lw.Wuk[kk], 256); cp(s.bk[kk], lw.bk[kk], 256);
+                cp(s.Wfk[kk], lw.Wfk[kk], 96); cp(s.bg[kk + 1], lw.bgk[kk], 32);
+              }
+              cp(s.bg[0], lw.bg0, 32); cp(s.wa, lw.wa, 256); cp(s.ba, lw.ba, 1);
+            });
           } else {
             const int last = layer == q.L - 1;
             const LayerW wn = q.layers[last ? layer : layer + 1];
             SmallWR4& s = reinterpret_cast<NodeTail*>(tail)->sw;
-            uint32_t total = sz(1024) + sz(192) + sz(512) + sz(32) + 2 * sz(256) + sz(256) + sz(96) + sz(8) + 2 * sz(256) + sz(1);
-            total += last ? sz(1024) + sz(96) + sz(d.Hin) : sz(256) + 2 * sz(32 * hid0) + 2 * sz(96);
-            mbar_expect_tx(&B.wbar, total);
-            auto cp = [&](float* dst, const float* src, int n) { bulk_g2s(dst, src, sz(n), &B.wbar); };
-            cp(s.Wdf, lw.Wdf, 64 * 16); cp(s.Wff, lw.Wff, 64 * 3); cp(s.Wuf, lw.Wuf, 16 * 32); cp(s.bgf, lw.bgf, 32);
-            cp(s.b1, lw.b1, 256); cp(s.b2, lw.b2, 256);
-            cp(s.Wdp, lw.Wdp, 32 * 8); cp(s.Wfp, lw.Wfp, 32 * 3); cp(s.Wup, lw.Wup, 8); cp(s.bp, lw.bp, 256);
-            cp(s.wgp, lw.Wgp, 256); cp(s.bgp, lw.bgp, 1);
-            if (!last) {
-              cp(s.u.nx.b0, wn.b0, 256);
-              cp(s.u.nx.Wd0i, wn.Wd0i, 32 * hid0); cp(s.u.nx.Wd0j, wn.Wd0j, 32 * hid0);
-              cp(s.u.nx.Wf0i, wn.Wf0i, 96); cp(s.u.nx.Wf0j, wn.Wf0j, 96);
-            } else {
-              cp(s.u.pj.pWd, ew.pWd, 32 * 32); cp(s.u.pj.pWf, ew.pWf, 96); cp(s.u.pj.pbs, ew.pbs, d.Hin);
-            }
+            stage([&](auto&& cp) {
+              cp(s.Wdf, lw.Wdf, 64 * 16); cp(s.Wff, lw.Wff, 64 * 3); cp(s.Wuf, lw.Wuf, 16 * 32); cp(s.bgf, lw.bgf, 32);
+              cp(s.b1, lw.b1, 256); cp(s.b2, lw.b2, 256);
+              cp(s.Wdp, lw.Wdp, 32 * 8); cp(s.Wfp, lw.Wfp, 32 * 3); cp(s.Wup, lw.Wup, 8); cp(s.bp, lw.bp, 256);
+              cp(s.wgp, lw.Wgp, 256); cp(s.bgp, lw.bgp, 1);
+              if (!last) {
+                cp(s.u.nx.b0, wn.b0, 256);
+                cp(s.u.nx.Wd0i, wn.Wd0i, 32 * hid0); cp(s.u.nx.Wd0j, wn.Wd0j, 32 * hid0);
+                cp(s.u.nx.Wf0i, wn.Wf0i, 96); cp(s.u.nx.Wf0j, wn.Wf0j, 96);
+              } else {
+                cp(s.u.pj.pWd, ew.pWd, 32 * 32); cp(s.u.pj.pWf, ew.pWf, 96); cp(s.u.pj.pbs, ew.pbs, d.Hin);
+              }
+            });
           }
         }
         mbar_wait(&B.wbar, pw);
@@ -337,22 +337,18 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
       // next publish follows directly; publish: a GEMM phase whose accumulators the epilogue reads after the barrier
       auto run = [&]() __attribute__((always_inline)) { fence_proxy_async(); named_bar_sync(3, TC_EPI); PH(); gemm(ph++); };
       auto publish = [&]() __attribute__((always_inline)) { run(); named_bar_sync(3, TC_EPI); PH(); };
-      auto wait_d = [&]() __attribute__((always_inline)) {};
       // node tile: U has been read (E3a), so G4 may overwrite its columns
       auto release_u = [&]() __attribute__((always_inline)) { named_bar_sync(3, TC_EPI); gemm(-1); named_bar_sync(3, TC_EPI); };
       if (type == 0) {
         EdgeTail& T = *reinterpret_cast<EdgeTail*>(tail);
         const int half = tid >> 7, r = tid & 127;
         const SmallW& sw = T.sw;
-        (void)release_u;
 #include "edge_tile_epilogue.inc"
       } else {
         NodeTail& T = *reinterpret_cast<NodeTail*>(tail);
         NodeScratch& SC = *reinterpret_cast<NodeScratch*>(X + R5_BLOCKS * R5_BLOCK);
         const int l = lane, s = warp, c0 = warp * 32;
         const SmallWR4& sw = T.sw;
-        (void)T;
-        (void)run;
 #include "node_r4_tile_epilogue.inc"
       }
       PH();

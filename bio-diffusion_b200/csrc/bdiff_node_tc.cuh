@@ -14,13 +14,17 @@ constexpr int NM_S = 0, NM_U = 256;
 constexpr int R4M = 32;
 constexpr int NM_S1 = 256;        // second accumulator (overlaps U, see G4)
 
-// bytes of one layer's node-pass weight stream (see k_pack_node_slabs for the order)
-__host__ __device__ inline size_t tc_node_stream_bytes(int last) {
-  const size_t s256 = 2 * 256 * 32, s288 = 2 * 288 * 32, s32 = 2 * 32 * 32;
-  size_t b = 16 * s256 + 16 * s288 + 2 * s256 + 16 * s256 + 16 * s288;      // G1a G1b G1c G2 G3a
-  b += last ? 2 * s256 + 19 * s32 : 16 * s256 + 2 * s256 + 16 * s256;       // G3b Gp | G4 G3b G5
-  return b;
+// Node pass weight stream (StreamSeg / Stream: bdiff_edge_tc.cuh), in issue order; the last layer has no next layer to
+// prepare (G4, G5) and ends with the projection instead.
+//   G1a: W1[0:256]   G1b: W1[256:512] + 16 gate rows of -Wg_ff   G1c: W1[512:544]   G2: W2   G3a: Wp[0:256] + 16 gate rows of Wg_ff
+//   G4: next.Wsi   G3b: Wp[256:288]   G5: next.Wsj   Gp: projection scalar_out (K = 300 -> 19 steps, Hin -> 32 rows, zero padded)
+enum { NG_1A, NG_1B, NG_1C, NG_2, NG_3A, NG_4, NG_3B, NG_5, NGL_3B = 5, NGL_P = 6 };     // NGL_*: the last layer's tail
+__host__ __device__ constexpr Stream tc_node_stream(bool last) {
+  constexpr StreamSeg G{16, 128, 1}, Gg{16, 144, 1}, Gx{2, 128, 1};
+  return last ? Stream{{G, Gg, Gx, G, Gg, Gx, {19, 16, 4}}, 7} : Stream{{G, Gg, Gx, G, Gg, G, Gx, G}, 8};
 }
+static_assert(stream_max_chunk(tc_node_stream(false)) <= TC_SLOT && stream_max_chunk(tc_node_stream(true)) <= TC_SLOT,
+              "a node-pass chunk must fit a ring slot");
 
 // the small weights with the (mutually exclusive) next-layer / projection sets overlaid
 struct alignas(16) SmallWR4 {
@@ -44,7 +48,6 @@ struct NodeScratch {
   float sVD[R4M][49];      // vector_down of the feed-forward GCP (16 x 3)
   float sVP[R4M][25];      // vector_down of the position GCP (8 x 3)
   float sDot[8][R4M];
-  int2 sMid[R4M];          // per node {first middle edge tile, count} of its row (n > 128 only), see Plan::node_mid
 };
 static_assert(R5_BLOCKS * (size_t)R5_BLOCK + sizeof(NodeScratch) <= XE_BLOCKS * (size_t)X_BLOCK, "node scratch must fit behind the R5 blocks");
 

@@ -61,7 +61,7 @@ __device__ __forceinline__ void selftest_gemm(uint32_t xa, uint32_t wb, bool r5,
   acc_store<N>(d, n0, threadIdx.x >> 7);
 }
 
-__global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __restrict__ A,
+__global__ void __launch_bounds__(320, 1) k_wgmma_selftest_split(const float* __restrict__ A,
                                                                  const unsigned char* __restrict__ wimg,
                                                                  float* __restrict__ scratch, float* __restrict__ C,
                                                                  int variant) {
@@ -70,12 +70,12 @@ __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __r
   unsigned char* X = smem;                           // edge layout: hi blocks 0,1 | lo blocks 2,3;  R5 layout: 2 blocks x 20 KiB
   unsigned char* Wb = smem + 4 * X_BLOCK;
   uint64_t* bars = reinterpret_cast<uint64_t*>(Wb + (size_t)ST_STEPS * 2 * ST_SLAB);
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const bool r5 = variant & 2;
   if (tid == 0) {
     mbar_init(&bars[0], 1);
     mbar_fence_init();
-    tm_base = scratch;
+    acc_scratch = scratch;
   }
   __syncthreads();
   if (tid < 128) {
@@ -110,17 +110,16 @@ __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __r
     selftest_gemm<32, -1>(xa, wb, r5, 288);
     named_bar_sync(3, 256);
     const int half = tid >> 7, r = tid & 127;
-    const uint32_t tl = (uint32_t)((warp & 3) * 32) << 16;
     // pair exchange through the scratch: each half writes 8 values into its own columns, reads the partner's
     float mine[8], theirs[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) mine[i] = (float)(1000 * half + r * 8 + i);
-    tmem_st8(tl + 320 + half * 8, mine);
+    scratch_st<8>(320 + half * 8, mine);
     named_bar_sync(3, 256);
-    tmem_ld8(tl + 320 + (half ^ 1) * 8, theirs);
+    scratch_ld<8>(320 + (half ^ 1) * 8, theirs);
     for (int c0 = half * 160; c0 < half * 160 + 160; c0 += 32) {
       float v[32];
-      tmem_ld32(tl + c0, v);
+      scratch_ld<32>(c0, v);
 #pragma unroll
       for (int i = 0; i < 32; ++i) C[(size_t)r * 336 + c0 + i] = v[i];
     }
@@ -131,13 +130,13 @@ __global__ void __launch_bounds__(320, 1) k_umma_selftest_split(const float* __r
 
 
 cudaError_t selftest_configure() {
-  return cudaFuncSetAttribute(k_umma_selftest_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ST_SMEM);
+  return cudaFuncSetAttribute(k_wgmma_selftest_split, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ST_SMEM);
 }
 
-void launch_umma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
+void launch_wgmma_selftest_split(cudaStream_t st, const float* A, const float* W, unsigned char* img_scratch, float* C,
                                 int variant) {
   k_selftest_pack_slabs<<<(ST_N * ST_K + 255) / 256, 256, 0, st>>>(W, img_scratch);
-  k_umma_selftest_split<<<1, 320, ST_SMEM, st>>>(A, img_scratch, reinterpret_cast<float*>(img_scratch + ST_IMG), C, variant);
+  k_wgmma_selftest_split<<<1, 320, ST_SMEM, st>>>(A, img_scratch, reinterpret_cast<float*>(img_scratch + ST_IMG), C, variant);
 }
 
 size_t selftest_img_bytes() { return ST_IMG + (size_t)TM_COLS * 128 * sizeof(float); }

@@ -7,8 +7,8 @@
 //   node tile  : 5 blocks of [160 rows][64] ("R5"): node l of the 32-node tile is stored as hi in rows l, l+64, l+128
 //                and as lo in rows l+32, l+96.  The MMA reads the block through two 128-row views (row 0: hi lo hi lo,
 //                row 32: lo hi lo hi); view0.W_hi + view32.W_hi + view0.W_lo + view32.W_lo leaves the complete
-//                (hi+lo)(W_hi+W_lo) product in all four row quarters of the accumulator, so the 8 compute warps keep sharing the 32
-//                nodes exactly as in the row-replicated bf16 kernel of round 1.
+//                (hi+lo)(W_hi+W_lo) product in all four row quarters of the accumulator, so the 8 compute warps share the 32
+//                nodes: each reads its accumulator columns from its own row quarter.
 // B operand (weights, packed once per weight update): "slabs" of one K=16 step:
 //                [hi plane | lo plane], plane = [2 K-chunks][N rows][16 bytes], un-swizzled (SWIZZLE_NONE, LBO = N*16,
 //                SBO = 128).  A slab plane is one contiguous TMA bulk copy of N*32 bytes (<= 10 KiB for N = 320), which
@@ -39,9 +39,6 @@ __device__ __forceinline__ void x_store8_hl(unsigned char* X, int lo0, int r, in
 
 // ---- edge tile (9 blocks)
 constexpr int XE_LO = 4, XE_EXTRA = 8, XE_BLOCKS = 9;
-__device__ __forceinline__ void xe_store8(unsigned char* X, int r, int kk, const float* v) {   // kk % 8 == 0, kk < 256
-  x_store8_hl(X, XE_LO, r, kk, v);
-}
 __device__ __forceinline__ void xe_store4(unsigned char* X, int r, int kk, float a, float b, float c, float d) {   // kk % 4 == 0
   uint32_t h0, l0, h1, l1;
   split_bf16x2(a, b, h0, l0);
@@ -56,13 +53,6 @@ __device__ __forceinline__ void xe_store1(unsigned char* X, int r, int kk, float
   const uint32_t off = sw128_offset(r, kk & 63);
   *reinterpret_cast<__nv_bfloat16*>(X + (kk >> 6) * X_BLOCK + off) = hi;
   *reinterpret_cast<__nv_bfloat16*>(X + (XE_LO + (kk >> 6)) * X_BLOCK + off) = lo;
-}
-__device__ __forceinline__ void xe_load8(const unsigned char* X, int r, int kk, float* v) {   // kk % 8 == 0, kk < 256
-  const uint32_t off = sw128_offset(r, kk & 63);
-  const uint4 h = *reinterpret_cast<const uint4*>(X + (kk >> 6) * X_BLOCK + off);
-  const uint4 l = *reinterpret_cast<const uint4*>(X + (XE_LO + (kk >> 6)) * X_BLOCK + off);
-  const float2 a = join_bf16x2(h.x, l.x), b = join_bf16x2(h.y, l.y), c = join_bf16x2(h.z, l.z), e = join_bf16x2(h.w, l.w);
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; v[4] = c.x; v[5] = c.y; v[6] = e.x; v[7] = e.y;
 }
 // extra block: column c in [0,32): hi at k = c, lo at k = 32 + c
 __device__ __forceinline__ void xe_store8_extra(unsigned char* X, int r, int c, const float* v) {   // c % 8 == 0

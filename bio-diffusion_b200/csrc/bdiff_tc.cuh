@@ -7,7 +7,7 @@
 //     SBO = 1024 B (8 rows), layout SWIZZLE_128B.  A warpgroup's M=64 rows start 64*128 = 8 KiB further on.
 //   B: un-swizzled K=16 slabs (see bdiff_slab.cuh), descriptor with explicit LBO / SBO.
 //   Accumulators: registers of the issuing warpgroup, stored at the end of a GEMM phase to a per-CTA scratch of 128 rows
-//   x 512 columns (column-major) that the epilogue threads read by row; scratch addresses are (row << 16) | column.
+//   x 512 columns (column-major) that the epilogue threads read by row (scratch_ld / scratch_st).
 //   Elementwise epilogues instead run on the registers themselves (frag_row / frag_col give each register's place).
 #pragma once
 #include <cuda_bf16.h>
@@ -96,10 +96,7 @@ __device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
 
 // ------------------------------------------------------------------------------------------ accumulator scratch
 // Base of this CTA's [512 columns][128 rows] fp32 scratch; set by the kernel before its first barrier.
-__shared__ float* tm_base;
-__device__ __forceinline__ float* tm_word(uint32_t taddr) {
-  return tm_base + (size_t)(taddr & 0xffffu) * 128 + (taddr >> 16) + (threadIdx.x & 31);
-}
+__shared__ float* acc_scratch;
 // wgmma fragment of an M=64 x N tile issued by warpgroup wg: register j of this thread holds the element at row
 // frag_row(wg, j) of the 128-row tile and column frag_col(j) of the tile's N columns.  Registers j and j + 1 (j even)
 // are two adjacent columns of one row.
@@ -110,95 +107,41 @@ __device__ __forceinline__ int frag_col(int j) { return 8 * (j >> 2) + 2 * (thre
 // fragment (columns col0 ..) <-> scratch
 template <int N>
 __device__ __forceinline__ void acc_store(const float* d, int col0, int wg) {
-  float* const base = tm_base;     // one read of the pointer (a store through float* could alias it)
+  float* const base = acc_scratch;     // one read of the pointer (a store through float* could alias it)
 #pragma unroll
   for (int j = 0; j < N / 2; ++j) base[(size_t)(col0 + frag_col(j)) * 128 + frag_row(wg, j)] = d[j];
 }
 template <int N>
 __device__ __forceinline__ void acc_load(float* d, int col0, int wg) {
-  const float* const base = tm_base;
+  const float* const base = acc_scratch;
 #pragma unroll
   for (int j = 0; j < N / 2; ++j) d[j] = base[(size_t)(col0 + frag_col(j)) * 128 + frag_row(wg, j)];
 }
 
-// scratch -> registers: this thread's row (32*(warp%4) + laneid, encoded in taddr's upper half), `N` consecutive columns
-__device__ __forceinline__ void tmem_ld8_nw(uint32_t taddr, uint32_t* r) {
-  const float* p = tm_word(taddr);
+// This thread's row of the scratch: row 32 * (warp % 4) + lane, columns col .. col + N - 1.  Nothing here orders the
+// accesses of different threads: that is the job of the CTA barriers around them.
+__device__ __forceinline__ float* scratch_row() { return acc_scratch + (threadIdx.x & 127); }
+template <int N>
+__device__ __forceinline__ void scratch_ld(int col, float* v) {
+  const float* p = scratch_row() + (size_t)col * 128;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) r[i] = __float_as_uint(p[i * 128]);
+  for (int i = 0; i < N; ++i) v[i] = p[i * 128];
 }
-__device__ __forceinline__ void tmem_ld32_nw(uint32_t taddr, uint32_t* r) {
-  const float* p = tm_word(taddr);
+template <int N>
+__device__ __forceinline__ void scratch_st(int col, const float* v) {
+  float* p = scratch_row() + (size_t)col * 128;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(p[i * 128]);
+  for (int i = 0; i < N; ++i) p[i * 128] = v[i];
 }
-__device__ __forceinline__ void tmem_ld_wait() {}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-  const float* p = tm_word(taddr);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = p[i * 128];
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  const float* p = tm_word(taddr);
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = p[i * 128];
-}
-__device__ __forceinline__ void tmem_st8_nw(uint32_t taddr, const float* v) {
-  float* p = tm_word(taddr);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) p[i * 128] = v[i];
-}
-__device__ __forceinline__ void tmem_st_wait() {}
-template <int N8>
-__device__ __forceinline__ void tmem_ld8xN(uint32_t taddr, float* v) {
-  const float* p = tm_word(taddr);
-#pragma unroll
-  for (int i = 0; i < N8 * 8; ++i) v[i] = p[i * 128];
-}
-template <int N8>
-__device__ __forceinline__ void tmem_st8xN(uint32_t taddr, const float* v) {
-#pragma unroll
-  for (int q = 0; q < N8; ++q) tmem_st8_nw(taddr + q * 8, v + q * 8);
-}
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, float* v) { tmem_ld8xN<8>(taddr, v); }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) { tmem_st8_nw(taddr, v); }
-// Ordering of scratch accesses between threads is given by the CTA barriers around them; these mark the places.
-__device__ __forceinline__ void tc_fence_before() {}
-__device__ __forceinline__ void tc_fence_after() {}
 
-// The packed fp32x2 intrinsics of sm_100 (__fmul2_rn & co.) are not available when compiling device code for sm_90:
-// two-lane versions with the same names, one instruction per lane (the host pass sees the toolkit's declarations).
+// Two-lane fp32 arithmetic, one instruction per lane.  The names are those of the toolkit's packed fp32x2 intrinsics,
+// which exist for device code from sm_100 on only (the host pass sees the toolkit's declarations); sm_90 device code gets
+// these definitions.
 #if defined(__CUDA_ARCH__) && __CUDA_ARCH__ < 1000
 __device__ __forceinline__ float2 __fmul2_rn(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 __device__ __forceinline__ float2 __fadd2_rn(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 __ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 #endif
-
-// fast activations for the tensor path (one MUFU each; operands are rounded to bf16 anyway)
-__device__ __forceinline__ float tanh_fast(float x) {
-  float y;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
-__device__ __forceinline__ float silu_fast(float x) { return x * sigmoid_fast(x); }
-
-// packed fp32x2 versions (two lanes per call)
-__device__ __forceinline__ float2 sigmoid_fast2(float2 x) {
-  const float2 hx = __fmul2_rn(x, make_float2(0.5f, 0.5f));
-  const float2 t = make_float2(tanh_fast(hx.x), tanh_fast(hx.y));
-  return __ffma2_rn(t, make_float2(0.5f, 0.5f), make_float2(0.5f, 0.5f));
-}
-__device__ __forceinline__ float2 silu_fast2(float2 x) { return __fmul2_rn(x, sigmoid_fast2(x)); }
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
-  __nv_bfloat162 h = *reinterpret_cast<__nv_bfloat162*>(&u);
-  return __bfloat1622float2(h);
-}
 
 // ------------------------------------------------------------------------------------- split-bf16 operands
 // Every GEMM operand of the tensor path is the pair (hi, lo) of bf16 numbers with hi = RN_bf16(value)
@@ -221,8 +164,8 @@ __device__ __forceinline__ void split_bf16(float a, __nv_bfloat16& hi, __nv_bflo
   lo = __float2bfloat16_rn(a - __bfloat162float(hi));
 }
 
-// fp32-class activations for the tensor path: ex2.approx / rcp.approx are accurate to ~2 ulp (the former
-// tanh.approx form was good to 2^-11 only).  sigmoid(x) = 1 / (1 + 2^(-x log2 e)).
+// fp32-class activations for the tensor path: ex2.approx / rcp.approx are accurate to ~2 ulp.
+// sigmoid(x) = 1 / (1 + 2^(-x log2 e)).
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -244,18 +187,6 @@ __device__ __forceinline__ float2 silu_acc2(float2 x) { return __fmul2_rn(x, sig
 
 // A-operand tile: 128 rows x 64 bf16 per K-block (16 KiB), K-blocks consecutive.
 constexpr int X_BLOCK = 128 * 128;
-__device__ __forceinline__ void x_store8(unsigned char* X, int r, int kk, const float* v) {   // kk % 8 == 0
-  *reinterpret_cast<uint4*>(X + (kk >> 6) * X_BLOCK + sw128_offset(r, kk & 63)) =
-      make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-}
-__device__ __forceinline__ void x_store1(unsigned char* X, int r, int kk, float v) {
-  *reinterpret_cast<__nv_bfloat16*>(X + (kk >> 6) * X_BLOCK + sw128_offset(r, kk & 63)) = __float2bfloat16_rn(v);
-}
-__device__ __forceinline__ void x_load8(const unsigned char* X, int r, int kk, float* v) {
-  const uint4 u = *reinterpret_cast<const uint4*>(X + (kk >> 6) * X_BLOCK + sw128_offset(r, kk & 63));
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), e = unpack_bf16x2(u.w);
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y; v[4] = c.x; v[5] = c.y; v[6] = e.x; v[7] = e.y;
-}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

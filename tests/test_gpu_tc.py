@@ -28,7 +28,7 @@ CHAIN_TOL = 1e-3
 
 
 @pytest.mark.parametrize("variant", [0, 2])
-def test_umma_selftest_split_matches_fp64_matmul(variant):
+def test_wgmma_selftest_split_matches_fp64_matmul(variant):
     """variant 0: edge-tile layout (hi / lo A blocks, 3 products); variant 2: node-tile R5 layout (2 row views, 4 products)."""
     import bdiff
     lib = bdiff.load_library()
@@ -45,8 +45,8 @@ def test_umma_selftest_split_matches_fp64_matmul(variant):
     ref = aa @ w.double().t()
     ref[:, 288:] = -ref[:, 288:]
     err = (c[:, :320].double() - ref).abs().max().item() / ref.abs().max().item()
-    print(f"split-bf16 UMMA self test variant {variant}: rel err vs fp64 {err:.3e}")
-    assert err < 3e-5, f"UMMA self test rel err {err:.3e}"
+    print(f"split-bf16 wgmma self test variant {variant}: rel err vs fp64 {err:.3e}")
+    assert err < 3e-5, f"wgmma self test rel err {err:.3e}"
     r = torch.arange(128, device="cuda", dtype=torch.float32)[:, None] * 8 + torch.arange(8, device="cuda")[None, :]
     assert torch.equal(c[:, 320:328], 1000 + r) and torch.equal(c[:, 328:336], r)      # accumulator-scratch pair exchange
 

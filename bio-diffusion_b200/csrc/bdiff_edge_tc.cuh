@@ -10,8 +10,8 @@ constexpr int TMT = 128;                 // edges per tile
 // weight ring: TC_NSLOT slots of TC_SLOT bytes; a chunk is always a single contiguous TMA bulk copy
 constexpr int TC_SLOT = 2 * 160 * 32;    // 10 KiB: one N half of the widest K step (checked against the stream tables)
 constexpr int TC_NSLOT = 5;
-// accumulator-scratch column map of an edge tile (512 columns)
-constexpr int TM_S = 0, TM_U0 = 256, TM_U1 = 288, TM_MV = 320, TM_VD0 = 416;
+// accumulator-scratch column map of an edge tile (512 columns; S never leaves the registers, so columns 0..255 are unused)
+constexpr int TM_U0 = 256, TM_U1 = 288, TM_MV = 320, TM_VD0 = 416;
 constexpr int TM_EX = 416, TM_EX_STRIDE = 40;     // pair-exchange scratch (over VD0, which is dead by then): 2 x 40 columns
 
 // ---- The weight stream of one (pass, layer), defined here and nowhere else: the pack kernels (bdiff_tc_pack.cu), the
@@ -49,11 +49,12 @@ __host__ __device__ constexpr int tc_k0_steps(int Ed, int Xd) {     // K=16 step
   return (Ed + (64 + Xd) / 4 + 9 + 15) / 16;
 }
 // Edge pass: entry i is GEMM phase i of edge_tile_mma.inc.
-//   G0: W0e, zero-padded to k0s * 16 K rows;  G(k)a, k = 1..3: [W_k rows | 32 gate rows: half 0 -> U0, half 1 -> U1];
-//   G(k)b: W_k K rows 256..287;  G4: Wg_3, four K steps per chunk.
+//   G0: W0e, zero-padded to k0s * 16 K rows;  G(k)u, k = 1..3: 32 gate rows of m_{k-1} (half 0 -> U0, half 1 -> U1),
+//   four K steps per chunk;  G(k)s: all K rows of W_k ([m_{k-1} | vn_k | q_k], zero-padded to 288);  G4: Wg_3, four K
+//   steps per chunk.
 __host__ __device__ constexpr Stream tc_edge_stream(int k0s) {
-  constexpr StreamSeg Ga{16, 160, 1}, Gb{2, 128, 1};
-  return {{{k0s, 128, 1}, Ga, Gb, Ga, Gb, Ga, Gb, {16, 16, 4}}, 8};
+  constexpr StreamSeg Gu{16, 32, 4}, Gs{18, 128, 1};
+  return {{{k0s, 128, 1}, Gu, Gs, Gu, Gs, Gu, Gs, {16, 16, 4}}, 8};
 }
 static_assert(stream_max_chunk(tc_edge_stream(8)) <= TC_SLOT, "an edge-pass chunk must fit a ring slot");
 

@@ -36,7 +36,7 @@ __device__ bool stream_find(const Stream& S, long long row, SlabPos& p) {
   return false;
 }
 
-// Edge pass (tc_edge_stream).  Gate rows of G(k)a: GCP k adds +Wg_{k-1} m_{k-1} to U[(k-1) & 1] and starts
+// Edge pass (tc_edge_stream).  Gate rows of G(k)u: GCP k adds +Wg_{k-1} m_{k-1} to U[(k-1) & 1] and starts
 // U[k & 1] = -Wg_k m_{k-1} (sign folded into the packed weights so that U0 | U1 is one N=64 accumulator range).
 // one thread per (global plane row, k in [0,16)); writes the hi and the lo plane element
 __global__ void k_pack_edge_slabs(LayerW lw, Dims d, unsigned char* __restrict__ blob, size_t half_bytes) {
@@ -53,15 +53,13 @@ __global__ void k_pack_edge_slabs(LayerW lw, Dims d, unsigned char* __restrict__
     v = lw.Wgk[2][(size_t)k * 32 + n];
   } else {
     const int gi = (p.seg - 1) >> 1;        // GCP gi + 1
-    if (!(p.seg & 1)) {                     // G(k)b
-      v = 256 + k < kKM ? lw.Wk[gi][(size_t)(256 + k) * 256 + n] : 0.f;
-    } else if (n < 256) {
-      v = lw.Wk[gi][(size_t)k * 256 + n];
-    } else {
+    if (!(p.seg & 1)) {                     // G(k)s
+      v = k < kKM ? lw.Wk[gi][(size_t)k * 256 + n] : 0.f;
+    } else {                                // G(k)u
       const float* wprev = gi == 0 ? lw.Wg0 : lw.Wgk[gi - 1];
       const float* wthis = lw.Wgk[gi];
       const bool odd = ((gi + 1) & 1) != 0;           // GCP odd: U0 <- +prev, U1 <- -this;  even: U0 <- -this, U1 <- +prev
-      const int c = (n - 256) & 31;
+      const int c = n & 31;
       v = (p.half == 0) == odd ? wprev[(size_t)k * 32 + c] : -wthis[(size_t)k * 32 + c];
     }
   }

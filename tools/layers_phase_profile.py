@@ -25,7 +25,7 @@ import gcpnet_oracle as O  # noqa: E402  (seeded weights only)
 # Phases between consecutive stamps, in stamp order (edge_tile_epilogue.inc / node_r4_tile_epilogue.inc: one stamp at the
 # tile's start, one before and one after every published GEMM phase, one at the tile's end).  The edge tile's E0 and
 # E(k)b run inside their GEMM phases (on the wgmma fragments), so those phases have no stamp between G and E.
-EDGE_PHASES = ("T0", "G0+E0", "G1a", "E1a", "G1b+E1b", "G2a", "E2a", "G2b+E2b", "G3a", "E3a", "G3b+E3b", "G4", "sum+E4")
+EDGE_PHASES = ("T0", "G0+E0", "G1u", "E1a", "G1s+E1b", "G2u", "E2a", "G2s+E2b", "G3u", "E3a", "G3s+E3b", "G4", "sum+E4")
 NODE_PHASES = ("T0a", "G1a", "T0v+T0b", "G1b/c", "E1", "G2", "E2", "G3a", "E3a+G4", "G3b", "E3b", "G5|Gp", "E4/E5|Ep")
 
 

@@ -7,6 +7,7 @@ Public surface (mirrors the reference's seam, SURVEY.md §8b):
     GCDMTrainLoss        training-mode L2 objective of the same function (value only, no backward)
     check_molecular_stability_batch   the reference's check_molecular_stability for a whole sampled batch in one kernel
     GCDMTrainTail        adaptive clipping + AdamW(amsgrad) + EMA of a training step as three multi-tensor kernels
+    PropertyClassifier   EDM's EGNN property classifier (inference), packed molecules, drop-in for get_classifier's model
     DenoiserConfig       dims derived from the reference's Hydra config groups
 """
 from .config import DenoiserConfig, parameter_shapes
@@ -15,7 +16,8 @@ from .sampler import GCDMSampler
 from .loss import GCDMEvalNLL, GCDMTrainLoss
 from .optim import GCDMTrainTail
 from .stability import check_molecular_stability_batch
+from .classifier import PropertyClassifier
 from .datasets import QM9_N_NODES, GEOM_N_NODES, sample_num_nodes
 from ._lib import BdiffError, load as load_library
 
-__all__ = ["DenoiserConfig", "parameter_shapes", "GCPNetDynamicsB200", "GCDMSampler", "GCDMEvalNLL", "GCDMTrainLoss", "GCDMTrainTail", "check_molecular_stability_batch", "QM9_N_NODES", "GEOM_N_NODES", "sample_num_nodes", "BdiffError", "load_library"]
+__all__ = ["DenoiserConfig", "parameter_shapes", "GCPNetDynamicsB200", "GCDMSampler", "GCDMEvalNLL", "GCDMTrainLoss", "GCDMTrainTail", "check_molecular_stability_batch", "PropertyClassifier", "QM9_N_NODES", "GEOM_N_NODES", "sample_num_nodes", "BdiffError", "load_library"]

@@ -25,6 +25,11 @@ class Config(C.Structure):
                 ("xi_hidden", C.c_int32), ("mode", C.c_int32)]
 
 
+class ClassifierConfig(C.Structure):
+    _fields_ = [("in_node_nf", C.c_int32), ("in_edge_nf", C.c_int32), ("hidden_nf", C.c_int32),
+                ("n_layers", C.c_int32), ("attention", C.c_int32), ("node_attr", C.c_int32)]
+
+
 # name -> (restype, argtypes): exactly the symbols include/bdiff.h declares
 PROTOTYPES = {
     "bdiff_abi_version": (C.c_int32, []),
@@ -69,6 +74,13 @@ PROTOTYPES = {
     "bdiff_train_backward": (C.c_int32, [C.c_void_p] * 4),
     "bdiff_nan_guard_count": (C.c_int32, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64), C.c_int32]),
     "bdiff_launch_count": (C.c_int64, [C.c_void_p]),
+    "bdiff_classifier_create": (C.c_int32, [C.POINTER(ClassifierConfig), C.POINTER(C.c_void_p)]),
+    "bdiff_classifier_destroy": (None, [C.c_void_p]),
+    "bdiff_classifier_last_error": (C.c_char_p, [C.c_void_p]),
+    "bdiff_classifier_set_weight": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_char_p, C.c_void_p, C.POINTER(C.c_int64),
+                                                C.c_int32]),
+    "bdiff_classifier_forward": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

@@ -285,6 +285,33 @@ BDIFF_API int32_t bdiff_nan_guard_count(bdiff_handle* h, void* stream, int64_t* 
 /* Counters for bench.py: kernels launched by this handle since creation. */
 BDIFF_API int64_t bdiff_launch_count(const bdiff_handle* h);
 
+/* ---- EGNN property classifier (inference) -----------------------------------------------------------------------------
+ * Replaces: the EDM property classifier the QM9 property-conditional evaluation and the property-optimisation workload
+ * score molecules with — EGNN / E_GCL_mask / E_GCL (src/__init__.py:233-419), built by get_classifier (:97-114) and run by
+ * test_with_property_classifier (:144-230) on dense batches padded to the largest molecule.  Here molecules are packed
+ * (real atoms only): molecule k is atoms mol_off_host[k] .. mol_off_host[k+1] - 1 of x fp32[N,3] and one_hot fp32[N,5],
+ * 1 <= n_k <= 128.  bdiff_classifier_forward writes pred fp32[B], the normalised property (EGNN.forward's output); it
+ * copies mol_off to the device (the only host work) and never synchronises.  Supported: in_node_nf 5, in_edge_nf 0,
+ * hidden_nf 128, either attention and node_attr; anything else -> BDIFF_EINVAL.  set_weight takes the reference's
+ * parameter names (embedding.*, gcl_{i}.edge_mlp.{0,2}.*, gcl_{i}.node_mlp.{0,2}.*, gcl_{i}.att_mlp.0.*, node_dec.{0,2}.*,
+ * graph_dec.{0,2}.*) as contiguous fp32 device tensors and repacks them on `stream`.  Results are bit-reproducible. */
+typedef struct bdiff_classifier bdiff_classifier;
+typedef struct bdiff_classifier_config {
+  int32_t in_node_nf;   /* 5   */
+  int32_t in_edge_nf;   /* 0   */
+  int32_t hidden_nf;    /* nf: 128 */
+  int32_t n_layers;     /* 1..64 */
+  int32_t attention;    /* 0 / 1 */
+  int32_t node_attr;    /* 0 / 1 */
+} bdiff_classifier_config;
+BDIFF_API int32_t bdiff_classifier_create(const bdiff_classifier_config* cfg, bdiff_classifier** out);
+BDIFF_API void bdiff_classifier_destroy(bdiff_classifier* h);
+BDIFF_API const char* bdiff_classifier_last_error(const bdiff_classifier* h);   /* h may be NULL: last creation error */
+BDIFF_API int32_t bdiff_classifier_set_weight(bdiff_classifier* h, void* stream, const char* name, const float* data,
+                                              const int64_t* shape, int32_t ndim);
+BDIFF_API int32_t bdiff_classifier_forward(bdiff_classifier* h, void* stream, int32_t num_mols, const int32_t* mol_off_host,
+                                           const float* x, const float* one_hot, float* pred);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,8 +19,6 @@
 //
 // The TMA-producer lane also claims the tiles (so the next tile's weights stream while the current tile computes) and hands
 // them to the flag lane and the 8 compute warps through a two-slot mbarrier ring.
-#include <type_traits>
-
 #include "bdiff_node_tc.cuh"
 
 namespace bdiff {
@@ -52,101 +50,6 @@ constexpr int LAYERS_THREADS = 384;
 constexpr int LAYERS_REG_COMPUTE = 232, LAYERS_REG_SERVICE = 40;
 static_assert(256 * LAYERS_REG_COMPUTE + 128 * LAYERS_REG_SERVICE <= 168 * LAYERS_THREADS, "setmaxnreg pool");
 constexpr int RING_CONSUMERS = TC_EPI / 32;       // one arrival per compute warp frees a ring slot
-
-// One ring chunk c of a GEMM phase: issue(ts, tu, chunk address, c) issues its wgmmas into fresh register tiles (ts: NS
-// columns; tu: TU tiles of NU columns, for chunks that carry TU K steps whose products must stay apart), one wait, the
-// slot is released, and the tiles are added to the running sums s / u with round-to-nearest fp32 adds, tile after tile:
-// the tensor core's own fp32 accumulation truncates, and over a 1000-step chain (where |h| grows by ~17 decades) that
-// bias towards zero compounds into a visible drift from the fp32 path.
-template <int NS, int NU, int TU, class Issue>
-__device__ __forceinline__ void seg_chunk(TcBars& B, uint32_t raddr, uint32_t& ci, int c, float* s, float* u, Issue& issue) {
-  constexpr int RS = NS ? NS / 2 : 1, RU = NU ? NU / 2 : 1;
-  const uint32_t slot = ci % TC_NSLOT;
-  float ts[RS], tu[TU * RU];
-#pragma unroll
-  for (int i = 0; i < RS; ++i) ts[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < TU * RU; ++i) tu[i] = 0.f;
-  mbar_wait(&B.full[slot], (ci / TC_NSLOT) & 1);
-  wgmma_fence();
-  issue(ts, tu, raddr + slot * TC_SLOT, c);
-  wgmma_commit();
-  wgmma_wait<0>();
-  acc_fence<RS>(ts);
-  acc_fence<TU * RU>(tu);
-  mbar_arrive_if(&B.empty[slot], (threadIdx.x & 31) == 0);
-  ++ci;
-  if (NS) {
-#pragma unroll
-    for (int i = 0; i < RS; ++i) s[i] += ts[i];
-  }
-  if (NU) {
-#pragma unroll
-    for (int t = 0; t < TU; ++t)
-#pragma unroll
-      for (int i = 0; i < RU; ++i) u[i] += tu[t * RU + i];
-  }
-}
-
-// One weight-stream segment of a GEMM phase, run by both compute warpgroups (warpgroup wg: tile rows [64 wg, 64 wg + 64)).
-// For each N half h of the weight planes, `nch` = seg_chunks(stream-table entry) ring chunks (seg_chunk) into the
-// accumulators s (NS columns, scratch columns scol + h NS) and u (NU columns at ucol + h NU), which start at zero (s:
-// sfresh; u: bit h of ufresh) or from the scratch.  A finished half goes to the scratch, or, when an epilogue
-// `epi(s, u, h, wg)` is given, to that functor (fragment layout: frag_row / frag_col), which then runs between the
-// halves' wgmmas: it must be always_inline and free of divergent branches (see the kernel's note on C7520).
-struct AccToScratch {};
-template <int NS, int NU, int TU = 1, class Issue, class Epi = AccToScratch>
-__device__ __forceinline__ void run_seg(TcBars& B, uint32_t raddr, uint32_t& ci, int nch, int scol, bool sfresh, int ucol,
-                                        int ufresh, Issue&& issue, Epi&& epi = Epi{}) {
-  constexpr int RS = NS ? NS / 2 : 1, RU = NU ? NU / 2 : 1;
-  const int wg = threadIdx.x >> 7;
-  for (int h = 0; h < 2; ++h) {
-    float s[RS], u[RU];
-    if (NS) {
-      if (sfresh) {
-#pragma unroll
-        for (int i = 0; i < RS; ++i) s[i] = 0.f;
-      } else {
-        acc_load<NS>(s, scol + h * NS, wg);
-      }
-    }
-    if (NU) {
-      if ((ufresh >> h) & 1) {
-#pragma unroll
-        for (int i = 0; i < RU; ++i) u[i] = 0.f;
-      } else {
-        acc_load<NU>(u, ucol + h * NU, wg);
-      }
-    }
-    for (int c = 0; c < nch; ++c) seg_chunk<NS, NU, TU>(B, raddr, ci, c, s, u, issue);
-    if constexpr (std::is_same_v<std::decay_t<Epi>, AccToScratch>) {
-      if (NS) acc_store<NS>(s, scol + h * NS, wg);
-      if (NU) acc_store<NU>(u, ucol + h * NU, wg);
-    } else {
-      epi(s, u, h, wg);
-    }
-  }
-}
-
-// A segment of N = 2 x 128 columns that starts at zero and whose epilogue overwrites part of its own A operand: N half
-// 0's epilogue writes A columns that half 1's chunks 0..hold still read.  Half 0's finished accumulators therefore wait
-// in registers until this warpgroup has retired half 1's chunk `hold`; then epi(s, nullptr, 0, wg) runs, then the rest of
-// half 1 and epi(s, nullptr, 1, wg).  Same products and adds in the same order as run_seg<128, 0>.
-template <class Issue, class Epi>
-__device__ __forceinline__ void run_seg_held(TcBars& B, uint32_t raddr, uint32_t& ci, int nch, int hold, Issue&& issue,
-                                             Epi&& epi) {
-  const int wg = threadIdx.x >> 7;
-  float s0[64], s1[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) s0[i] = 0.f;
-  for (int c = 0; c < nch; ++c) seg_chunk<128, 0, 1>(B, raddr, ci, c, s0, nullptr, issue);
-#pragma unroll
-  for (int i = 0; i < 64; ++i) s1[i] = 0.f;
-  for (int c = 0; c <= hold; ++c) seg_chunk<128, 0, 1>(B, raddr, ci, c, s1, nullptr, issue);
-  epi(s0, nullptr, 0, wg);
-  for (int c = hold + 1; c < nch; ++c) seg_chunk<128, 0, 1>(B, raddr, ci, c, s1, nullptr, issue);
-  epi(s1, nullptr, 1, wg);
-}
 
 template <int ED, int XD>
 __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d, EmbedW ew, LayerSched q, Work w) {
@@ -278,32 +181,11 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
             list([&](float* dst, const float* src, int n) { bulk_g2s(dst, src, sz(n), &B.wbar); });
           };
           if (type == 0) {
-            SmallW& s = reinterpret_cast<EdgeTail*>(tail)->sw;
-            stage([&](auto&& cp) {
-              cp(s.Wd0x, lw.Wd0x, XD * HID0); cp(s.Wf0x, lw.Wf0x, XD * 3); cp(s.Wu0, lw.Wu0, HID0 * 32);
-              for (int kk = 0; kk < 3; ++kk) {
-                cp(s.Wdk[kk], lw.Wdk[kk], 256); cp(s.Wuk[kk], lw.Wuk[kk], 256); cp(s.bk[kk], lw.bk[kk], 256);
-                cp(s.Wfk[kk], lw.Wfk[kk], 96); cp(s.bg[kk + 1], lw.bgk[kk], 32);
-              }
-              cp(s.bg[0], lw.bg0, 32); cp(s.wa, lw.wa, 256); cp(s.ba, lw.ba, 1);
-            });
+            stage([&](auto&& cp) { small_w_copies<XD>(reinterpret_cast<EdgeTail*>(tail)->sw, lw, cp); });
           } else {
             const int last = layer == q.L - 1;
             const LayerW wn = q.layers[last ? layer : layer + 1];
-            SmallWR4& s = reinterpret_cast<NodeTail*>(tail)->sw;
-            stage([&](auto&& cp) {
-              cp(s.Wdf, lw.Wdf, 64 * 16); cp(s.Wff, lw.Wff, 64 * 3); cp(s.Wuf, lw.Wuf, 16 * 32); cp(s.bgf, lw.bgf, 32);
-              cp(s.b1, lw.b1, 256); cp(s.b2, lw.b2, 256);
-              cp(s.Wdp, lw.Wdp, 32 * 8); cp(s.Wfp, lw.Wfp, 32 * 3); cp(s.Wup, lw.Wup, 8); cp(s.bp, lw.bp, 256);
-              cp(s.wgp, lw.Wgp, 256); cp(s.bgp, lw.bgp, 1);
-              if (!last) {
-                cp(s.u.nx.b0, wn.b0, 256);
-                cp(s.u.nx.Wd0i, wn.Wd0i, 32 * hid0); cp(s.u.nx.Wd0j, wn.Wd0j, 32 * hid0);
-                cp(s.u.nx.Wf0i, wn.Wf0i, 96); cp(s.u.nx.Wf0j, wn.Wf0j, 96);
-              } else {
-                cp(s.u.pj.pWd, ew.pWd, 32 * 32); cp(s.u.pj.pWf, ew.pWf, 96); cp(s.u.pj.pbs, ew.pbs, d.Hin);
-              }
-            });
+            stage([&](auto&& cp) { small_wr4_copies(reinterpret_cast<NodeTail*>(tail)->sw, lw, wn, ew, hid0, d.Hin, last, cp); });
           }
         }
         mbar_wait(&B.wbar, pw);

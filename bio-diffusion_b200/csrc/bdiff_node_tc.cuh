@@ -36,6 +36,23 @@ struct alignas(16) SmallWR4 {
     struct { float pWd[32 * 32], pWf[32 * 3], pbs[32]; } pj;
   } u;
 };
+// every (destination, source, float count) that fills SmallWR4 for a node tile of the layer lw, as cp(dst, src, n):
+// the next layer's set from wn, or in the last layer (wn unused) the projection set from ew
+template <class Copy>
+__device__ __forceinline__ void small_wr4_copies(SmallWR4& s, const LayerW& lw, const LayerW& wn, const EmbedW& ew, int hid0,
+                                                 int hin, bool last, Copy&& cp) {
+  cp(s.Wdf, lw.Wdf, 64 * 16); cp(s.Wff, lw.Wff, 64 * 3); cp(s.Wuf, lw.Wuf, 16 * 32); cp(s.bgf, lw.bgf, 32);
+  cp(s.b1, lw.b1, 256); cp(s.b2, lw.b2, 256);
+  cp(s.Wdp, lw.Wdp, 32 * 8); cp(s.Wfp, lw.Wfp, 32 * 3); cp(s.Wup, lw.Wup, 8); cp(s.bp, lw.bp, 256);
+  cp(s.wgp, lw.Wgp, 256); cp(s.bgp, lw.bgp, 1);
+  if (!last) {
+    cp(s.u.nx.b0, wn.b0, 256);
+    cp(s.u.nx.Wd0i, wn.Wd0i, 32 * hid0); cp(s.u.nx.Wd0j, wn.Wd0j, 32 * hid0);
+    cp(s.u.nx.Wf0i, wn.Wf0i, 96); cp(s.u.nx.Wf0j, wn.Wf0j, 96);
+  } else {
+    cp(s.u.pj.pWd, ew.pWd, 32 * 32); cp(s.u.pj.pWf, ew.pWf, 96); cp(s.u.pj.pbs, ew.pbs, hin);
+  }
+}
 
 struct NodeTail : TcBars {
   SmallWR4 sw;

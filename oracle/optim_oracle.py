@@ -78,3 +78,33 @@ class TrainTailOracle:
             self.ema[i].sub_(diff)
         self.last = {"norm": norm, "limit": limit, "coef": coef}
         return self.last
+
+
+# ------------------------------------------------------------------ gradients of tests/golden/optim_long.pt
+# (drawn from numpy's PCG64 generator, the same numbers on every machine, so the fixture need not store them)
+LONG_SIZES = [1, 3, 16384, 16385, 32773]
+LONG_RUNS = [  # queue_len, amsgrad, steps, {step: gradient scale} of the spikes (every other step: scale 0.5 .. 2)
+    (1, True, 14, {5: 4.0, 9: 60.0}),
+    (3, False, 16, {7: 3.0, 11: 80.0}),
+    (50, True, 64, {53: 3.0, 58: 200.0}),
+    (120, True, 134, {123: 3.0, 127: 50.0, 130: 1.0}),
+]
+
+
+def long_run_grads(queue_len, steps, spikes):
+    """Initial parameters, then for every step the gradient of every tensor (float32, seeded by queue_len)."""
+    rng = np.random.default_rng(4000 + queue_len)
+    init = [torch.from_numpy(rng.standard_normal(n, dtype=np.float32) * np.float32(0.1)) for n in LONG_SIZES]
+    grads = []
+    for k in range(steps):
+        sc = np.float32(spikes.get(k, 0.5 + 1.5 * rng.random()))
+        grads.append([torch.from_numpy(rng.standard_normal(n, dtype=np.float32) * sc) for n in LONG_SIZES])
+    return init, grads
+
+
+def fingerprint_index(n, chunk=16384):
+    """Entries of an n-element tensor that optim_long.pt stores: both ends, +-4 around every chunk border, every 97th."""
+    idx = set(range(min(n, 8))) | set(range(max(0, n - 8), n)) | set(range(0, n, 97))
+    for b in range(chunk, n, chunk):
+        idx |= set(range(b - 4, min(n, b + 4)))
+    return torch.tensor(sorted(idx), dtype=torch.int64)

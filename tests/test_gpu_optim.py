@@ -43,6 +43,57 @@ def test_train_tail_matches_oracle_and_fixture():
     assert opt.kernel_launches == 3 * len(fx["grads"])
 
 
+def _check_fingerprint(got, fp, rtol, atol, what):
+    g = got.detach().reshape(-1).cpu()
+    assert torch.allclose(g[OO.fingerprint_index(g.numel())], fp["vals"], rtol=rtol, atol=atol), what
+    assert abs(float(g.double().norm()) - fp["norm"]) <= rtol * fp["norm"] + atol, what
+
+
+@pytest.mark.parametrize("run", range(4))
+def test_train_tail_past_the_history_window(run):
+    """GCDMTrainTail for more than queue_len + 10 steps (queue_len 1, 3, 50, 120), gradient spikes after the seeded 3000 has
+    left the history, chunk-edge tensor sizes, one run without amsgrad: against the reference's pieces (optim_long.pt)
+    every step and at the end, and against TrainTailOracle on every element."""
+    from bdiff.optim import GCDMTrainTail
+    fx = torch.load(os.path.join(GOLDEN, "optim_long.pt"), weights_only=False)
+    assert fx["sizes"] == OO.LONG_SIZES
+    r = fx["runs"][run]
+    init, grads = OO.long_run_grads(r["queue_len"], r["steps"], r["spikes"])
+    assert len(grads) > r["queue_len"] + 10
+    params = [torch.nn.Parameter(p.clone().cuda()) for p in init]
+    opt = GCDMTrainTail(params, amsgrad=r["amsgrad"], queue_len=r["queue_len"])
+    orc = OO.TrainTailOracle(init, amsgrad=r["amsgrad"], queue_len=r["queue_len"])
+    for k, (gs, ref) in enumerate(zip(grads, r["log"])):
+        opt.zero_grad()
+        for p, g in zip(params, gs):
+            p.grad.add_(g.cuda())
+        opt.step()
+        o = orc.step(gs)
+        rep = opt.report()
+        assert abs(rep["norm"] - ref["norm"]) <= 2e-6 * ref["norm"], f"step {k}: norm"
+        assert abs(rep["limit"] - ref["limit"]) <= 2e-6 * ref["limit"], f"step {k}: limit"
+        assert rep["clipped"] == ref["clipped"], f"step {k}: clipped"
+        assert abs(rep["coef"] - o["coef"]) <= 2e-6, f"step {k}: coef"
+        assert len(rep["history"]) == min(k + 2, r["queue_len"]), f"step {k}: history length"
+    assert any(l["clipped"] for l in r["log"][r["queue_len"] + 1:]), "no clipping after the seed left the history"
+    assert opt.report()["step"] == r["steps"]
+    for i, (got, a, fp) in enumerate(zip(params, orc.p, r["params"])):
+        assert torch.allclose(got.detach().cpu(), a, rtol=2e-6, atol=1e-8), f"parameter {i}"
+        _check_fingerprint(got, fp, 2e-6, 1e-8, f"parameter {i}")
+    for i, (got, a, fp) in enumerate(zip(opt.ema_parameters(), orc.ema, r["ema"])):
+        assert torch.allclose(got.cpu(), a, rtol=2e-6, atol=1e-8), f"EMA {i}"
+        _check_fingerprint(got, fp, 2e-6, 1e-8, f"EMA {i}")
+    if r["amsgrad"]:
+        for i, (got, a, fp) in enumerate(zip(opt.max_exp_avg_sq, orc.vmax, r["max_exp_avg_sq"])):
+            assert torch.allclose(got.cpu(), a, rtol=5e-5, atol=1e-12), f"max_exp_avg_sq {i}"
+            _check_fingerprint(got, fp, 5e-5, 1e-12, f"max_exp_avg_sq {i}")
+    else:
+        assert opt.max_exp_avg_sq is None
+    hist = opt.report()["history"]
+    assert len(hist) == len(r["history"]) and max(abs(x - y) for x, y in zip(hist, r["history"])) <= 1e-2
+    assert 3000.0 not in hist
+
+
 def test_train_tail_rejects_cpu_and_replaced_grads():
     import bdiff
     from bdiff.optim import GCDMTrainTail

@@ -7,9 +7,9 @@ one window, crosses window borders (joined by `finish_crossing`), is cut by one 
 `agg`), or a tile lies strictly inside it (the tile's sum goes to `Work::mid`, the node tile adds those in ascending order).
 The schedule adds ghost tiles for odd tile counts, node tiles without edges and dependency ranges spanning molecules.
 
-LAYOUTS names batches that reach each of these paths.  `layout_paths` restates the tiling rules in plain Python; the CPU
-test checks that every case reaches what it claims and that the catalogue as a whole reaches every path class.  The GPU
-tests run every case through tensor mode, parity mode and the training forward and compare each molecule's coordinate and
+LAYOUTS names batches that reach each of these paths.  `layout_paths` restates the tiling rules in plain Python (both
+live in layout_catalogue.py, shared with the training-step tests of test_gpu_train_layouts.py); the CPU test checks that
+every case reaches what it claims and that the catalogue as a whole reaches every path class.  The GPU tests run every case through tensor mode, parity mode and the training forward and compare each molecule's coordinate and
 `h` blocks separately with the oracle in float64, each scaled by max(1, |ref|max) of that molecule and block, so that a
 small molecule next to a large one is held to its own scale.
 
@@ -17,101 +17,15 @@ Molecules without active atoms: the reference divides 0 by 0 for their centroid,
 velocity of the whole batch.  The CUDA path takes that centroid as 0 (DESIGN.md §2), so the oracle runs with
 guard_empty=True here; the empty molecule's own rows must be finite and agree between the two modes.
 """
-from dataclasses import dataclass, field
-from typing import List, Optional, Tuple
-
-import numpy as np
 import pytest
 import torch
 
 import gcpnet_oracle as O
-
-TMT = 128         # edges per edge tile (bdiff_edge_tc.cuh, TMT)
-WIN = 16          # rows per segmented-sum window, one warp each (edge_tile_epilogue.inc, wr0 = warp * 16)
-R4M = 32          # atoms per node tile (bdiff_node_tc.cuh, R4M)
+from layout_catalogue import BY_NAME, LAYOUTS, Layout, _active_mol_rows, _inputs, _offsets, layout_paths
 
 TENSOR_TOL = 1e-4   # tensor mode (split-bf16 wgmma), as tests/test_gpu_tc.py
 PARITY_TOL = 5e-5   # parity mode and the training forward (fp32), as tests/test_gpu_parity.py / test_gpu_train.py
 WEIGHT_SEED = {"qm9": 7, "qm9_cond": 5, "geom": 3}
-
-
-@dataclass
-class Layout:
-    name: str
-    config: str
-    sizes: List[int]
-    masked: List[int] = field(default_factory=list)     # masked atom indices (into the concatenated atom list)
-    targets: Tuple[str, ...] = ()                        # path classes this case is here to reach
-    schedule: bool = False                               # run through profile_forward: a timed-out dependency wait fails
-    scale: float = 1.0                                   # weight scale of the oracle comparisons (see below)
-
-    @property
-    def n(self):
-        return sum(self.sizes)
-
-    def mask(self) -> torch.Tensor:
-        m = torch.ones(self.n, dtype=torch.bool)
-        m[self.masked] = False
-        return m
-
-
-def _offsets(sizes):
-    return np.concatenate(([0], np.cumsum(sizes))).astype(int)
-
-
-def _mask_mols(sizes, mols):
-    """Every atom of molecules `mols`."""
-    o = _offsets(sizes)
-    return [i for k in mols for i in range(o[k], o[k + 1])]
-
-
-def _fuzz(config, seed):
-    """Fixed-seed random sizes (QM9 1..29, GEOM 1..60 atoms), about 10 % of the atoms masked, 3k..20k edges."""
-    rng = np.random.default_rng(1000 + seed + (0 if config == "qm9" else 100))
-    hi = 29 if config == "qm9" else 60
-    target = int(rng.integers(3000, 20000))
-    sizes = []
-    while sum(s * s for s in sizes) < target:
-        sizes.append(int(rng.integers(1, hi + 1)))
-    n = sum(sizes)
-    masked = sorted(int(i) for i in np.nonzero(rng.random(n) < 0.1)[0])
-    return Layout(f"fuzz_{config}_{seed}", config, sizes, masked, ("row cut once", "masked atom"))
-
-
-def _sparse(config):
-    # [12, 5, 45, 20]: interior masks in molecule 0; molecule 1 has one active atom; molecule 2 (atoms 17..61) keeps its
-    # first 5 atoms only, and molecule 3's first two atoms are masked, so node tile 1 (atoms 32..63) has no active atom
-    sizes = [12, 5, 45, 20]
-    masked = [3, 7, 8] + [12, 13, 15, 16] + list(range(22, 62)) + [62, 63, 70]
-    return Layout(f"sparse_mask_{config}", config, sizes, masked,
-                  ("masked atom", "one active atom", "node tile without active atoms"))
-
-
-# The untrained network amplifies round-off with the row length: with full-size random weights, the oracle's own float32
-# result misses the float64 one by 8e-5 .. 5e-4 (scaled) on the 128..300-atom molecules, so those cases run with
-# half-size weights (float32 vs float64 then within 5e-7), as the teacher-forced steps of test_gpu_parity.py do.
-LAYOUTS = [
-    Layout("ascending_1_to_29", "qm9", list(range(1, 30)), [],
-           ("row inside one window", "row crosses 1 window border", "row crosses 2+ window borders", "row cut once")),
-    Layout("row_is_tile", "qm9", [128], [], ("whole-tile row", "row crosses 7 window borders"), scale=0.5),
-    Layout("cut_1_127", "qm9", [1, 128], [], ("row cut 1 + 127",), scale=0.5),
-    Layout("two_mids", "geom", [1, 258, 3, 300], [], ("2 mid tiles",), scale=0.5),
-    Layout("mid_phases", "geom", [130, 131, 129, 181], [], ("1 mid tile", "row cut once"), scale=0.5),
-    Layout("empty_mols_qm9", "qm9", [3, 5, 4, 1, 6], _mask_mols([3, 5, 4, 1, 6], [0, 2, 4]),
-           ("empty molecule",)),
-    Layout("empty_mols_geom", "geom", [40, 27, 64, 50, 33], _mask_mols([40, 27, 64, 50, 33], [0, 2, 4]),
-           ("empty molecule", "empty node tile", "masked atom in the GEOM build")),
-    _sparse("qm9"),
-    _sparse("geom"),
-    Layout("node_tile_edges", "geom", [31, 2, 33, 70, 40, 17], [],
-           ("odd TN", "molecule straddles a node tile border", "molecule spans 3 node tiles"), schedule=True),
-    Layout("tiny_1", "qm9", [1], [], ("E = 1",), schedule=True),
-    Layout("tiny_2", "qm9", [2], [], ("odd TE",), schedule=True),
-    Layout("all_masked", "qm9", [3, 4], list(range(7)), ("E = 0",), schedule=True),
-    Layout("cond_masked", "qm9_cond", [9, 14, 20, 7], [2, 11, 12, 30, 40, 48], ("masked atom",)),
-] + [_fuzz(c, s) for c in ("qm9", "geom") for s in range(3)]
-
-BY_NAME = {c.name: c for c in LAYOUTS}
 
 # every path class the catalogue as a whole must reach
 PATH_CLASSES = {
@@ -121,72 +35,6 @@ PATH_CLASSES = {
     "empty node tile", "node tile without active atoms", "masked atom", "masked atom in the GEOM build",
     "one active atom", "molecule straddles a node tile border", "molecule spans 3 node tiles",
 }
-
-
-def layout_paths(sizes, mask, config="qm9"):
-    """The paths of k_layers_tc that a batch reaches, from the kernel's tiling rules (see the module docstring)."""
-    mask = np.asarray(mask, dtype=bool)
-    o = _offsets(sizes)
-    paths = set()
-    e = 0                          # first edge of the current molecule
-    tile_mols = {}                 # edge tile -> molecules with edges in it
-    for k in range(len(sizes)):
-        act = mask[o[k]:o[k + 1]]
-        na = int(act.sum())
-        if na == 0:
-            paths.add("empty molecule")
-        if na == 1 and sizes[k] > 1:
-            paths.add("one active atom")
-        if na < sizes[k]:
-            paths.add("masked atom")
-            if config == "geom":
-                paths.add("masked atom in the GEOM build")
-        if o[k] // R4M != (o[k + 1] - 1) // R4M:
-            paths.add("molecule straddles a node tile border")
-        if (o[k + 1] - 1) // R4M - o[k] // R4M >= 2:
-            paths.add("molecule spans 3 node tiles")
-        for a in range(na):
-            g0 = e + a * na
-            g1 = g0 + na - 1
-            t0, t1 = g0 // TMT, g1 // TMT
-            for t in range(t0, t1 + 1):
-                tile_mols.setdefault(t, set()).add(k)
-            if t1 == t0:
-                if g0 % TMT == 0 and g1 % TMT == TMT - 1:
-                    paths.add("whole-tile row")
-            elif t1 == t0 + 1:
-                paths.add("row cut once")
-                if (t1 * TMT - g0, g1 - t1 * TMT + 1) in ((1, TMT - 1), (TMT - 1, 1)):
-                    paths.add("row cut 1 + 127")
-            else:
-                paths.add(f"{t1 - t0 - 1} mid tile" + ("s" if t1 - t0 > 2 else ""))
-            # window borders crossed by each tile's piece of the row (tile borders are not window crossings)
-            for t in range(t0, t1 + 1):
-                a0, a1 = max(g0, t * TMT), min(g1, t * TMT + TMT - 1)
-                c = a1 // WIN - a0 // WIN
-                paths.add("row inside one window" if c == 0 else
-                          "row crosses 1 window border" if c == 1 else "row crosses 2+ window borders")
-                if c == TMT // WIN - 1:
-                    paths.add("row crosses 7 window borders")
-        e += na * na
-    te, tn = (e + TMT - 1) // TMT, (o[-1] + R4M - 1) // R4M
-    paths.add("odd TE" if te % 2 else "even TE")
-    paths.add("odd TN" if tn % 2 else "even TN")
-    if e == 0:
-        paths.add("E = 0")
-    if e == 1:
-        paths.add("E = 1")
-    if any(len(m) > 1 for m in tile_mols.values()):
-        paths.add("edge tile spans molecules")
-    mol_of = np.repeat(np.arange(len(sizes)), sizes)
-    for u in range(tn):
-        lo, hi = u * R4M, min(o[-1], u * R4M + R4M)
-        if not mask[lo:hi].any():
-            paths.add("node tile without active atoms")
-        # node_dep of bdiff_plan_topology: the edges of the molecules mol_of[lo] .. mol_of[hi - 1]
-        if all(mask[o[k]:o[k + 1]].sum() == 0 for k in range(mol_of[lo], mol_of[hi - 1] + 1)):
-            paths.add("empty node tile")
-    return paths
 
 
 def test_layout_catalogue_reaches_every_path():
@@ -240,33 +88,7 @@ def test_oracle_empty_molecule_guard():
                        O.denoiser_forward(sd, ocfg, bi, mask, xh, t, ctx, dtype=torch.float64, guard_empty=True))
 
 
-# ------------------------------------------------------------------------------------------------ inputs and oracle
-def _inputs(c: Layout):
-    """Seeded inputs of a case: masked xh rows are zero, coordinates centred per molecule, t and context per molecule."""
-    ocfg = O.config_named(c.config)
-    g = torch.Generator().manual_seed(sum(map(ord, c.name)))
-    b = len(c.sizes)
-    bi = torch.repeat_interleave(torch.arange(b), torch.tensor(c.sizes))
-    mask = c.mask()
-    xh = torch.randn((c.n, 3 + ocfg.num_h), generator=g) * mask[:, None]
-    _, xc = O.centralize(xh[:, :3], bi, mask, b, guard_empty=True)
-    xh = torch.cat((xc, xh[:, 3:]), -1)
-    t = torch.rand((b, 1), generator=g)[bi]
-    ctx = torch.randn((b, ocfg.num_context), generator=g)[bi] if ocfg.num_context else None
-    return bi, mask, xh, t, ctx
-
-
-def _active_mol_rows(c: Layout) -> torch.Tensor:
-    """Rows of molecules with at least one active atom."""
-    mask = c.mask()
-    o = _offsets(c.sizes)
-    keep = torch.zeros(c.n, dtype=torch.bool)
-    for k in range(len(c.sizes)):
-        if mask[o[k]:o[k + 1]].any():
-            keep[o[k]:o[k + 1]] = True
-    return keep
-
-
+# ------------------------------------------------------------------------------------------------ oracle
 _ORACLE = {}
 
 

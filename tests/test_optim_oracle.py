@@ -37,3 +37,27 @@ def test_queue_is_fifo_of_fifty():
     for v in range(10):
         q.add(v)
     assert q.items == [9.0, 8.0, 7.0, 6.0, 5.0]
+
+
+def test_oracle_matches_reference_pieces_past_the_history_window():
+    """optim_long.pt (queue_len 1, 3, 50, 120; spikes after the seeded 3000 has left the history; one run without amsgrad)."""
+    fx = torch.load(os.path.join(GOLDEN, "optim_long.pt"), weights_only=False)
+    assert fx["sizes"] == OO.LONG_SIZES and len(fx["runs"]) == len(OO.LONG_RUNS)
+    for r in fx["runs"]:
+        init, grads = OO.long_run_grads(r["queue_len"], r["steps"], r["spikes"])
+        o = OO.TrainTailOracle(init, amsgrad=r["amsgrad"], queue_len=r["queue_len"])
+        for grads_k, ref in zip(grads, r["log"]):
+            got = o.step(grads_k)
+            assert abs(got["norm"] - ref["norm"]) <= 1e-5 * ref["norm"]
+            assert abs(got["limit"] - ref["limit"]) <= 1e-6 * ref["limit"]
+            assert (got["norm"] > got["limit"]) == ref["clipped"]
+        assert any(l["clipped"] for l in r["log"][r["queue_len"] + 1:])
+        arrays = [("params", o.p, 1e-6, 1e-8), ("ema", o.ema, 1e-6, 1e-8)]
+        if r["amsgrad"]:
+            arrays.append(("max_exp_avg_sq", o.vmax, 1e-5, 1e-12))
+        for what, got, rtol, atol in arrays:
+            for a, fp in zip(got, r[what]):
+                assert torch.allclose(a[OO.fingerprint_index(a.numel())], fp["vals"], rtol=rtol, atol=atol), what
+                assert abs(float(a.double().norm()) - fp["norm"]) <= rtol * fp["norm"] + atol, what
+        assert len(o.queue.items) == r["queue_len"] and 3000.0 not in o.queue.items
+        assert max(abs(x - y) for x, y in zip(sorted(o.queue.items), r["history"])) <= 1e-3

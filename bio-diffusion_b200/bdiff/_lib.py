@@ -81,6 +81,11 @@ PROTOTYPES = {
                                                 C.c_int32]),
     "bdiff_classifier_forward": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
                                              C.c_void_p, C.c_void_p]),
+    "bdiff_classifier_param_floats": (C.c_int64, [C.c_void_p]),
+    "bdiff_classifier_param_layout": (C.c_int32, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "bdiff_classifier_train_forward": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p,
+                                                   C.c_void_p, C.c_void_p]),
+    "bdiff_classifier_train_backward": (C.c_int32, [C.c_void_p] * 4),
 }
 
 _lib = None

@@ -5,7 +5,13 @@ workload (mol_gen_eval_conditional_qm9.py:299-315, mol_gen_eval_optimization_qm9
 Same parameter names and shapes as the reference, so EDM's `best_checkpoint.npy` loads with strict=True, and the same
 dense call `forward(h0, x, edges, edge_attr, node_mask, edge_mask, n_nodes)`, so `test_with_property_classifier` runs
 unchanged.  Every arithmetic step runs in libbdiff_sm90.so (`bdiff_classifier_forward`) on packed molecules; `predict`
-takes the sampler's packed output directly.  Inference only: there is no CPU / PyTorch fallback and no backward.
+takes the sampler's packed output directly.  There is no CPU / PyTorch fallback.
+
+Under autograd (`torch.is_grad_enabled()` and some parameter requires grad — the train branch of
+`train_with_property_classifier`, :144-204) `forward` and `predict` run the library's training pass instead:
+`bdiff_classifier_train_forward` keeps a tape, `loss.backward()` reaches `bdiff_classifier_train_backward` through a
+`torch.autograd.Function` and every parameter receives its gradient (x and h0 are data: they get none).  A torch optimiser
+steps the parameters in place; the next call repacks them (`sync_weights`).
 """
 from __future__ import annotations
 
@@ -50,6 +56,28 @@ def classifier_parameter_shapes(n_layers: int, attention: bool, node_attr: bool,
     return out
 
 
+class _ClassifierTrainFn(torch.autograd.Function):
+    """pred = classifier(params; x, one_hot) with the library's tape; backward = bdiff_classifier_train_backward."""
+
+    @staticmethod
+    def forward(ctx, clf, x, one_hot, off, *params):
+        pred = clf._run(x, one_hot, off, train=True)
+        ctx.clf = clf
+        ctx.tape_id = clf._tape_id
+        ctx.needs = tuple(p.requires_grad for p in params)
+        return pred
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_pred):
+        clf = ctx.clf
+        if ctx.tape_id != clf._tape_id:
+            raise _lib.BdiffError("PropertyClassifier keeps ONE training tape: a later forward under autograd replaced the "
+                                  "one this backward needs (call backward() before the next training forward)")
+        grads = clf._train_backward(d_pred)
+        return (None,) * 4 + tuple(g if need else None for g, need in zip(grads, ctx.needs))
+
+
 class PropertyClassifier(nn.Module):
     """EGNN(in_node_nf, in_edge_nf, hidden_nf, device, act_fn, n_layers, coords_weight, attention, node_attr) with the
     reference's constructor arguments; only in_node_nf = 5, in_edge_nf = 0, hidden_nf = 128 and SiLU are supported."""
@@ -78,6 +106,9 @@ class PropertyClassifier(nn.Module):
         self.reset_parameters()
         self._handle = None
         self._weights_key = None
+        self._layout = None          # training: name -> (offset, count) in the flat gradient buffer
+        self._grad_flat = None
+        self._tape_id = 0
         self.to(device)
 
     @classmethod
@@ -146,15 +177,13 @@ class PropertyClassifier(nn.Module):
         self._weights_key = key
 
     # ------------------------------------------------------------------------------------------ forward
-    def _no_grad_guard(self):
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
-            raise RuntimeError("PropertyClassifier is inference-only: call it under torch.no_grad() / inference_mode() or "
-                               "freeze its parameters (training the classifier is not supported)")
+    def wants_grad(self) -> bool:
+        return torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
 
     def predict(self, x: torch.Tensor, one_hot: torch.Tensor, num_nodes: torch.Tensor) -> torch.Tensor:
         """pred [B] (normalised property) of packed molecules: x [N, 3], one_hot [N, 5] (the sampler's out[:, :3] and
-        out[:, 3:8]), num_nodes [B] with 1 <= n <= 128 summing to N."""
-        self._no_grad_guard()
+        out[:, 3:8]), num_nodes [B] with 1 <= n <= 128 summing to N.  Under autograd with trainable parameters the
+        result carries a grad_fn (the training pass; its values are bit-identical to the inference kernels')."""
         nn_ = torch.as_tensor(num_nodes).reshape(-1).to("cpu", torch.int64)
         n = int(x.shape[0])
         if x.dim() != 2 or x.shape[1] != 3:
@@ -167,26 +196,65 @@ class PropertyClassifier(nn.Module):
             raise ValueError(f"a molecule has {int(nn_.max())} atoms: the classifier takes at most {MAX_ATOMS}")
         if not x.is_cuda:
             raise _lib.BdiffError("PropertyClassifier runs on CUDA tensors only (no CPU fallback)")
+        off = torch.zeros(int(nn_.numel()) + 1, dtype=torch.int32)
+        off[1:] = torch.cumsum(nn_, 0).to(torch.int32)
+        if self.wants_grad():
+            return _ClassifierTrainFn.apply(self, x, one_hot, off, *self.parameters())
+        return self._run(x, one_hot, off, train=False)
+
+    def _run(self, x, one_hot, off, train: bool) -> torch.Tensor:
+        """bdiff_classifier_forward (train = False) or bdiff_classifier_train_forward (keeps the tape)."""
         self.sync_weights()
         lib = _lib.load()
-        b = int(nn_.numel())
-        off = torch.zeros(b + 1, dtype=torch.int32)
-        off[1:] = torch.cumsum(nn_, 0).to(torch.int32)
+        b = int(off.numel()) - 1
         xc = x.detach().to(torch.float32).contiguous()
         oh = one_hot.detach().to(device=xc.device, dtype=torch.float32).contiguous()
         pred = torch.empty(b, dtype=torch.float32, device=xc.device)
-        self._check(lib.bdiff_classifier_forward(
-            self._handle, C.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream), b,
-            off.numpy().ctypes.data_as(C.POINTER(C.c_int32)), C.c_void_p(xc.data_ptr()), C.c_void_p(oh.data_ptr()),
-            C.c_void_p(pred.data_ptr())), "bdiff_classifier_forward")
+        fn, what = ((lib.bdiff_classifier_train_forward, "bdiff_classifier_train_forward") if train
+                    else (lib.bdiff_classifier_forward, "bdiff_classifier_forward"))
+        self._check(fn(self._handle, C.c_void_p(torch.cuda.current_stream(xc.device).cuda_stream), b,
+                       off.numpy().ctypes.data_as(C.POINTER(C.c_int32)), C.c_void_p(xc.data_ptr()),
+                       C.c_void_p(oh.data_ptr()), C.c_void_p(pred.data_ptr())), what)
+        if train:
+            self._tape_id += 1
         return pred
+
+    def param_layout(self) -> dict:
+        """name -> (offset, count) of every parameter in the library's flat gradient buffer (bdiff_classifier_param_layout)."""
+        if self._layout is None:
+            lib = _lib.load()
+            h = self._ensure_handle()
+            lay = {}
+            for name, _ in self.named_parameters():
+                off, cnt = C.c_int64(), C.c_int64()
+                self._check(lib.bdiff_classifier_param_layout(h, name.encode(), C.byref(off), C.byref(cnt)),
+                            f"bdiff_classifier_param_layout({name})")
+                lay[name] = (int(off.value), int(cnt.value))
+            self._layout = lay
+        return self._layout
+
+    def _train_backward(self, d_pred: torch.Tensor):
+        lib = _lib.load()
+        lay = self.param_layout()
+        d = d_pred.detach().to(torch.float32).contiguous()
+        if self._grad_flat is None or self._grad_flat.device != d.device:
+            self._grad_flat = torch.empty(int(lib.bdiff_classifier_param_floats(self._handle)), dtype=torch.float32,
+                                          device=d.device)
+        self._check(lib.bdiff_classifier_train_backward(
+            self._handle, C.c_void_p(torch.cuda.current_stream(d.device).cuda_stream), C.c_void_p(d.data_ptr()),
+            C.c_void_p(self._grad_flat.data_ptr())), "bdiff_classifier_train_backward")
+        g = self._grad_flat.clone()        # autograd may keep / accumulate into what we return; the flat buffer is reused
+        out = []
+        for name, p in self.named_parameters():
+            off, cnt = lay[name]
+            out.append(g[off:off + cnt].view(p.shape).to(p.dtype))
+        return out
 
     def forward(self, h0: torch.Tensor, x: torch.Tensor, edges=None, edge_attr=None, node_mask: torch.Tensor = None,
                 edge_mask: torch.Tensor = None, n_nodes: int = None) -> torch.Tensor:
         """The reference's dense call (EGNN.forward, src/__init__.py:405-419): h0 [B*n, 5], x [B*n, 3], node_mask
         [B*n, 1], edge_mask [B*n*n, 1] = node-mask outer product without the diagonal (the construction of both evaluation
         scripts); `edges` is not read.  Packs the real atoms on the device and runs the same kernels as `predict`."""
-        self._no_grad_guard()
         if edge_attr is not None:
             raise NotImplementedError("edge attributes are not supported")
         n_nodes = int(n_nodes)

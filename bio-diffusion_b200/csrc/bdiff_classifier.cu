@@ -64,6 +64,13 @@ __global__ void k_clf_pack_w2(const float* __restrict__ W, unsigned char* __rest
   const int n = idx / CH, k = idx - n * CH;
   slab_store(slab + (size_t)(k >> 4) * W2_STEP, CH, n, k & 15, W[idx]);
 }
+// the slabs of W2^T (B operand of the reverse sweep's da = dz2 . W2)
+__global__ void k_clf_pack_w2t(const float* __restrict__ W, unsigned char* __restrict__ slab) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= CH * CH) return;
+  const int n = idx / CH, k = idx - n * CH;
+  slab_store(slab + (size_t)(k >> 4) * W2_STEP, CH, n, k & 15, W[(size_t)k * CH + n]);
+}
 
 // ---------------------------------------------------------------------------------------------------- edge kernel
 struct ClfEdgeArgs {
@@ -293,6 +300,9 @@ struct ClfNodeArgs {
   int N, layer, L, node_attr;
   ClfLayer cur, nxt;
   ClfWeights g;
+  // training pass only (TAPE = true): h_out receives the layer's output (h is its input and is not overwritten), agg is
+  // the layer's own tape slice (read, not zeroed), and the pre-activations / SiLU outputs the reverse sweep reads
+  float *h_out, *v, *u, *q, *qs;
 };
 
 // layer < 0: embedding (EGNN.forward :407), then P / Q of layer 0.
@@ -300,6 +310,9 @@ struct ClfNodeArgs {
 //            kernel's red.add words); then P / Q of layer l + 1, or node_dec after the last layer (:415).
 // One [NT][K3_MAX] tile in shared memory: columns 0..127 hold h, 128..255 agg and then the hidden activation u,
 // 256..263 the one-hot h0 (node_attr).
+// TAPE = false is the inference kernel; TAPE = true (the training pass) runs the same arithmetic and also writes the tape
+// (ClfNodeArgs: h_out, v / u = node_mlp.0 pre-activation / SiLU, q / qs = node_dec.0 pre-activation / SiLU).
+template <bool TAPE>
 __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
   __shared__ __align__(16) float sIn[NT * K3_MAX];
   float* const sH = sIn;
@@ -317,7 +330,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
     __syncthreads();
     acc_init(acc, a.g.embB);
     tile_gemm(sU, K3_MAX, 8, a.g.embWt, acc);
-    acc_out(acc, sH, false, a.h, node0, a.N);
+    acc_out(acc, sH, false, TAPE ? a.h_out : a.h, node0, a.N);
   } else {
     for (int i = tid; i < NT * (CH / 4); i += NODE_THREADS) {
       const int n = i / (CH / 4), c = (i % (CH / 4)) * 4;
@@ -326,7 +339,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
         float4* ag = reinterpret_cast<float4*>(a.agg + (size_t)(node0 + n) * CH + c);
         hv = *reinterpret_cast<const float4*>(a.h + (size_t)(node0 + n) * CH + c);
         gv = *ag;
-        *ag = make_float4(0.f, 0.f, 0.f, 0.f);
+        if constexpr (!TAPE) *ag = make_float4(0.f, 0.f, 0.f, 0.f);
       }
       *reinterpret_cast<float4*>(sH + n * K3_MAX + c) = hv;
       *reinterpret_cast<float4*>(sU + n * K3_MAX + c) = gv;
@@ -336,7 +349,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
     acc_init(acc, a.cur.b3);
     tile_gemm(sIn, K3_MAX, a.node_attr ? 2 * CH + 8 : 2 * CH, a.cur.W3t, acc);
     __syncthreads();     // agg is read: u takes its columns
-    acc_out(acc, sU, true, nullptr, node0, a.N);
+    if constexpr (TAPE) acc_out(acc, nullptr, false, a.v, node0, a.N);
+    acc_out(acc, sU, true, TAPE ? a.u : nullptr, node0, a.N);
     __syncthreads();
     acc_init(acc, a.cur.b4);
     tile_gemm(sU, K3_MAX, CH, a.cur.W4t, acc);
@@ -348,7 +362,7 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
         for (int q = 0; q < 4; ++q) acc[n][q] = sH[(n0 + n) * K3_MAX + c0 + q] + acc[n][q];
     }
     __syncthreads();     // every thread has read its h entries before they are overwritten
-    acc_out(acc, sH, false, a.h, node0, a.N);
+    acc_out(acc, sH, false, TAPE ? a.h_out : a.h, node0, a.N);
   }
   __syncthreads();
   if (a.layer < a.L - 1) {
@@ -361,7 +375,8 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
   } else {
     acc_init(acc, a.g.nd1b);
     tile_gemm(sH, K3_MAX, CH, a.g.nd1t, acc);
-    acc_out(acc, sU, true, nullptr, node0, a.N);
+    if constexpr (TAPE) acc_out(acc, nullptr, false, a.q, node0, a.N);
+    acc_out(acc, sU, true, TAPE ? a.qs : nullptr, node0, a.N);
     __syncthreads();
     acc_init(acc, a.g.nd2b);
     tile_gemm(sU, K3_MAX, CH, a.g.nd2t, acc);
@@ -370,8 +385,11 @@ __global__ void __launch_bounds__(NODE_THREADS) k_clf_node(ClfNodeArgs a) {
 }
 
 // pred_k = graph_dec(sum_{i in k} node_dec(h_i)): one CTA per molecule, the atom sum in atom order per column.
+// TAPE: also the molecule sums s, the graph_dec.0 pre-activation w and its SiLU ws, [B][128] each.
+template <bool TAPE>
 __global__ void __launch_bounds__(CH) k_clf_readout(const float* __restrict__ nodeout, const int* __restrict__ mol_off,
-                                                    ClfWeights g, float* __restrict__ pred) {
+                                                    ClfWeights g, float* __restrict__ pred, float* __restrict__ s_t = nullptr,
+                                                    float* __restrict__ w_t = nullptr, float* __restrict__ ws_t = nullptr) {
   __shared__ float s[CH], u[CH];
   const int k = blockIdx.x, c = threadIdx.x;
   const int a0 = mol_off[k], a1 = mol_off[k + 1];
@@ -381,6 +399,11 @@ __global__ void __launch_bounds__(CH) k_clf_readout(const float* __restrict__ no
   __syncthreads();
   float v = g.gd1b[c];
   for (int q = 0; q < CH; ++q) v = fmaf(s[q], __ldg(g.gd1t + (size_t)q * CH + c), v);
+  if constexpr (TAPE) {
+    s_t[(size_t)k * CH + c] = acc;
+    w_t[(size_t)k * CH + c] = v;
+    ws_t[(size_t)k * CH + c] = silu_acc(v);
+  }
   u[c] = silu_acc(v) * g.gd2[c];
   __syncthreads();
   if (c == 0) {
@@ -391,6 +414,8 @@ __global__ void __launch_bounds__(CH) k_clf_readout(const float* __restrict__ no
 }
 
 }  // namespace bdiff
+
+#include "bdiff_classifier_train.cuh"
 
 // ---------------------------------------------------------------------------------------------------- C ABI
 using namespace bdiff;
@@ -405,6 +430,18 @@ struct bdiff_classifier {
   // workspace (grown on demand)
   void* ws = nullptr;
   size_t ws_bytes = 0;
+  // training pass: W2^T slabs, the canonical flat layout (name -> offset, count), one tape and the reverse sweep's scratch
+  unsigned char* w2tbuf = nullptr;
+  std::map<std::string, std::pair<int64_t, int64_t>> playout;
+  int64_t pfloats = 0;
+  void* tape = nullptr;
+  size_t tape_bytes = 0;
+  void* bws = nullptr;
+  size_t bws_bytes = 0;
+  bool tape_valid = false;
+  uint64_t weights_gen = 0, tape_weights_gen = 0;
+  int tape_B = 0, tape_N = 0;
+  long long tape_E = 0;
   int num_sms = 0;
   std::string err;
   int fail(int code, const char* fmt, ...) {
@@ -447,7 +484,7 @@ size_t layout(bdiff_classifier* h, bool assign) {
 
 // one repack step: transposed columns [col0, col0 + ncols) of a [rows][cols] tensor, or a plain copy (transpose of a
 // [n][1] bias is a copy), or the W2 slab
-struct ClfOp { float* dst; int col0, ncols; unsigned char* slab; };
+struct ClfOp { float* dst; int col0, ncols; unsigned char* slab; bool tr = false; };
 
 bool resolve(bdiff_classifier* h, const std::string& name, std::vector<ClfOp>& ops, int64_t& rows, int64_t& cols) {
   const int in3 = 2 * CH + (h->cfg.node_attr ? CIN : 0);
@@ -475,7 +512,12 @@ bool resolve(bdiff_classifier* h, const std::string& name, std::vector<ClfOp>& o
     return true;
   }
   if (rest == "edge_mlp.0.bias") { rows = CH; cols = 1; ops.push_back({w.b1, 0, 1, nullptr}); return true; }
-  if (rest == "edge_mlp.2.weight") { rows = CH; cols = CH; ops.push_back({nullptr, 0, 0, w.W2s}); return true; }
+  if (rest == "edge_mlp.2.weight") {
+    rows = CH; cols = CH;
+    ops.push_back({nullptr, 0, 0, w.W2s});
+    if (h->w2tbuf) ops.push_back({nullptr, 0, 0, h->w2tbuf + (size_t)l * W2_BYTES, true});
+    return true;
+  }
   if (rest == "edge_mlp.2.bias") { rows = CH; cols = 1; ops.push_back({w.b2, 0, 1, nullptr}); return true; }
   if (rest.rfind("node_mlp.0.", 0) == 0) return lin(w.W3t, w.b3, in3, CH, rest.substr(11));
   if (rest.rfind("node_mlp.2.", 0) == 0) return lin(w.W4t, w.b4, CH, CH, rest.substr(11));
@@ -484,14 +526,88 @@ bool resolve(bdiff_classifier* h, const std::string& name, std::vector<ClfOp>& o
   return false;
 }
 
-cudaError_t grow(bdiff_classifier* h, size_t bytes) {
-  if (bytes <= h->ws_bytes) return cudaSuccess;
-  if (h->ws) cudaFree(h->ws);
-  h->ws = nullptr;
-  h->ws_bytes = 0;
-  cudaError_t e = cudaMalloc(&h->ws, bytes);
-  if (e == cudaSuccess) h->ws_bytes = bytes;
+cudaError_t grow_buf(void*& buf, size_t& have, size_t bytes) {
+  if (bytes <= have) return cudaSuccess;
+  if (buf) cudaFree(buf);
+  buf = nullptr;
+  have = 0;
+  cudaError_t e = cudaMalloc(&buf, bytes);
+  if (e == cudaSuccess) have = bytes;
   return e;
+}
+cudaError_t grow(bdiff_classifier* h, size_t bytes) { return grow_buf(h->ws, h->ws_bytes, bytes); }
+
+// Bump allocator over one device buffer: 256-byte aligned float slices.
+struct Carve {
+  unsigned char* base;
+  size_t used = 0;
+  float* f(size_t n) {
+    float* r = base ? reinterpret_cast<float*>(base + used) : nullptr;
+    used += (n * sizeof(float) + 255) / 256 * 256;
+    return r;
+  }
+};
+
+// The tape of one training forward (B molecules, N atoms, L layers).  Per layer l: h[l] its input (h[L] the last output),
+// P / Q (edge_mlp.0 node halves), agg, v / u (node_mlp.0 pre-activation / SiLU); node_dec's q / qs; readout s / w / ws;
+// copies of x, one_hot and the offsets (the reverse sweep must not depend on the caller's buffers).
+struct ClfTape {
+  float *h, *P, *Q, *agg, *v, *u, *q, *qs, *nodeout, *s, *w, *ws, *x, *oh;
+  int* mol_off;
+  long long* pair_off;
+};
+size_t tape_carve(unsigned char* base, int L, int N, int B, ClfTape& t) {
+  Carve c{base};
+  const size_t nc = (size_t)N * CH, lnc = (size_t)L * nc, bc = (size_t)B * CH;
+  t.h = c.f(lnc + nc); t.P = c.f(lnc); t.Q = c.f(lnc); t.agg = c.f(lnc); t.v = c.f(lnc); t.u = c.f(lnc);
+  t.q = c.f(nc); t.qs = c.f(nc); t.nodeout = c.f(nc); t.s = c.f(bc); t.w = c.f(bc); t.ws = c.f(bc);
+  t.x = c.f((size_t)N * 3); t.oh = c.f((size_t)N * CIN);
+  t.mol_off = reinterpret_cast<int*>(c.f(B + 1));
+  t.pair_off = reinterpret_cast<long long*>(c.f(2 * (size_t)(B + 1)));
+  return c.used;
+}
+// Scratch of the reverse sweep.  Per atom: two dh buffers (ping-pong over layers), dv, dagg, dP, dQ, R, dy, dq; per
+// molecule dw, dS; per pair a, s, dz2, dz1 and dt; the weight-gradient chunk partials.
+constexpr long long WG_MAX_CHUNKS = 256;
+struct ClfBwdScratch {
+  float *dHa, *dHb, *dV, *dAgg, *dP, *dQ, *R, *dY, *dQd, *dWk, *dS, *A, *S, *DZ2, *DZ1, *DT, *part;
+};
+size_t bws_carve(unsigned char* base, int N, int B, long long E, ClfBwdScratch& t) {
+  Carve c{base};
+  const size_t nc = (size_t)N * CH, ec = (size_t)E * CH;
+  t.dHa = c.f(nc); t.dHb = c.f(nc); t.dV = c.f(nc); t.dAgg = c.f(nc); t.dP = c.f(nc); t.dQ = c.f(nc); t.R = c.f(nc);
+  t.dY = c.f(nc); t.dQd = c.f(nc); t.dWk = c.f((size_t)B * CH); t.dS = c.f((size_t)B * CH);
+  t.A = c.f(ec); t.S = c.f(ec); t.DZ2 = c.f(ec); t.DZ1 = c.f(ec); t.DT = c.f(E);
+  t.part = c.f((size_t)WG_MAX_CHUNKS * CH * (CH + 1));
+  return c.used;
+}
+
+// dW[o][col0 + k] = sum_rows G[row][o] X[row][k] (k < K), db[o * dbs] = sum_rows G[row][o]: fixed chunks of rows, then
+// the chunks in index order — the summation order depends on `rows` only.
+void wgrad(cudaStream_t st, float* part, const float* G, int ldg, const float* X, int ldx, int O, int K, long long rows,
+           float* dW, int ldw, int col0, float* db, int dbs) {
+  long long nchunks = std::max(1ll, std::min(WG_MAX_CHUNKS, (rows + 255) / 256));
+  const long long chunk = ((rows + nchunks - 1) / nchunks + 31) / 32 * 32;
+  nchunks = std::max(1ll, (rows + chunk - 1) / chunk);
+  ClfWgradArgs a{G, X, ldg, ldx, O, K, rows, chunk, part};
+  k_clf_wgrad<<<dim3((O + 31) / 32, (K + 1 + 31) / 32, (unsigned)nchunks), 256, 0, st>>>(a);
+  k_clf_wgrad_sum<<<(O * (K + 1) + 255) / 256, 256, 0, st>>>(part, (int)nchunks, O, K, dW, ldw, col0, db, dbs);
+}
+
+// host checks of a packed batch shared by the inference and the training forward: pair offsets, or an error message
+int check_batch(bdiff_classifier* h, int32_t num_mols, const int32_t* mol_off_host, std::vector<long long>& pair_off) {
+  for (const auto& kv : h->seen)
+    if (!kv.second) return h->fail(BDIFF_ESTATE, "parameter '%s' was never set", kv.first.c_str());
+  if (mol_off_host[0] != 0) return h->fail(BDIFF_EINVAL, "mol_off[0] must be 0");
+  pair_off.assign(num_mols + 1, 0);
+  for (int k = 0; k < num_mols; ++k) {
+    const int n = mol_off_host[k + 1] - mol_off_host[k];
+    if (n < 1 || n > CLF_MAX_ATOMS)
+      return h->fail(BDIFF_EINVAL, "molecule %d has %d atoms: the classifier takes 1..%d atoms per molecule", k, n, CLF_MAX_ATOMS);
+    pair_off[k + 1] = pair_off[k] + (long long)n * n;
+  }
+  if ((pair_off[num_mols] + CT - 1) / CT > (1ll << 30)) return h->fail(BDIFF_EINVAL, "batch too large");
+  return BDIFF_OK;
 }
 
 }  // namespace
@@ -528,12 +644,15 @@ int32_t bdiff_classifier_create(const bdiff_classifier_config* cfg, bdiff_classi
   const size_t nf = layout(h, false);
   cudaError_t e = cudaMalloc(&h->wbuf, nf * sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&h->w2buf, (size_t)cfg->n_layers * W2_BYTES);
+  if (e == cudaSuccess) e = cudaMalloc(&h->w2tbuf, (size_t)cfg->n_layers * W2_BYTES);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_clf_bwd_edge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_EDGE_SMEM);
   if (e == cudaSuccess) e = cudaMemset(h->wbuf, 0, nf * sizeof(float));
   if (e == cudaSuccess) e = cudaFuncSetAttribute(k_clf_edge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)EDGE_SMEM);
   if (e != cudaSuccess) {
     g_clf_create_error = std::string("bdiff_classifier_create: ") + cudaGetErrorString(e);
     if (h->wbuf) cudaFree(h->wbuf);
     if (h->w2buf) cudaFree(h->w2buf);
+    if (h->w2tbuf) cudaFree(h->w2tbuf);
     delete h;
     return BDIFF_ECUDA;
   }
@@ -546,6 +665,14 @@ int32_t bdiff_classifier_create(const bdiff_classifier_config* cfg, bdiff_classi
     if (cfg->attention) lin(p + "att_mlp.0");
   }
   lin("node_dec.0"); lin("node_dec.2"); lin("graph_dec.0"); lin("graph_dec.2");
+  // canonical flat layout of the parameters / gradients: ascending name order, each tensor at a multiple of 64 floats
+  for (const auto& kv : h->seen) {
+    std::vector<ClfOp> ops;
+    int64_t rows = 0, cols = 0;
+    resolve(h, kv.first, ops, rows, cols);
+    h->playout[kv.first] = {h->pfloats, rows * cols};
+    h->pfloats += (rows * cols + 63) / 64 * 64;
+  }
   *out = h;
   return BDIFF_OK;
 }
@@ -554,7 +681,10 @@ void bdiff_classifier_destroy(bdiff_classifier* h) {
   if (!h) return;
   if (h->wbuf) cudaFree(h->wbuf);
   if (h->w2buf) cudaFree(h->w2buf);
+  if (h->w2tbuf) cudaFree(h->w2tbuf);
   if (h->ws) cudaFree(h->ws);
+  if (h->tape) cudaFree(h->tape);
+  if (h->bws) cudaFree(h->bws);
   delete h;
 }
 
@@ -573,7 +703,9 @@ int32_t bdiff_classifier_set_weight(bdiff_classifier* h, void* stream, const cha
                    (long long)cols, (long long)got_rows, (long long)got_cols);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   for (const ClfOp& op : ops) {
-    if (op.slab) {
+    if (op.slab && op.tr) {
+      k_clf_pack_w2t<<<(CH * CH + 255) / 256, 256, 0, st>>>(data, op.slab);
+    } else if (op.slab) {
       k_clf_pack_w2<<<(CH * CH + 255) / 256, 256, 0, st>>>(data, op.slab);
     } else if (cols == 1 || rows == 1) {      // bias or single-row weight: a copy
       cudaMemcpyAsync(op.dst, data, (size_t)rows * cols * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -585,6 +717,7 @@ int32_t bdiff_classifier_set_weight(bdiff_classifier* h, void* stream, const cha
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "set_weight(%s): %s", name, cudaGetErrorString(e));
   it->second = true;
+  ++h->weights_gen;
   return BDIFF_OK;
 }
 
@@ -592,20 +725,11 @@ int32_t bdiff_classifier_forward(bdiff_classifier* h, void* stream, int32_t num_
                                  const float* x, const float* one_hot, float* pred) {
   if (!h) return BDIFF_EINVAL;
   if (num_mols < 1 || !mol_off_host || !x || !one_hot || !pred) return h->fail(BDIFF_EINVAL, "bad argument");
-  for (const auto& kv : h->seen)
-    if (!kv.second) return h->fail(BDIFF_ESTATE, "parameter '%s' was never set", kv.first.c_str());
-  if (mol_off_host[0] != 0) return h->fail(BDIFF_EINVAL, "mol_off[0] must be 0");
-  std::vector<long long> pair_off(num_mols + 1, 0);
-  for (int k = 0; k < num_mols; ++k) {
-    const int n = mol_off_host[k + 1] - mol_off_host[k];
-    if (n < 1 || n > CLF_MAX_ATOMS)
-      return h->fail(BDIFF_EINVAL, "molecule %d has %d atoms: the classifier takes 1..%d atoms per molecule", k, n, CLF_MAX_ATOMS);
-    pair_off[k + 1] = pair_off[k] + (long long)n * n;
-  }
+  std::vector<long long> pair_off;
+  if (const int rc = check_batch(h, num_mols, mol_off_host, pair_off)) return rc;
   const int N = mol_off_host[num_mols];
   const long long E = pair_off[num_mols];
   const long long ntiles = (E + CT - 1) / CT;
-  if (ntiles > (1ll << 30)) return h->fail(BDIFF_EINVAL, "batch too large");
   // workspace: h, P, Q, agg, nodeout [N][128] fp32 | mol_off int32 [B+1] | pair_off int64 [B+1]
   const size_t node_bytes = (size_t)N * CH * sizeof(float);
   const size_t off_i = 5 * node_bytes, off_p = off_i + ((size_t)(num_mols + 1) * 4 + 15) / 16 * 16;
@@ -641,11 +765,146 @@ int32_t bdiff_classifier_forward(bdiff_classifier* h, void* stream, int32_t num_
     na.layer = l;
     if (l >= 0) na.cur = h->layers[l];
     if (l + 1 < L) na.nxt = h->layers[l + 1];
-    k_clf_node<<<node_grid, NODE_THREADS, 0, st>>>(na);
+    k_clf_node<false><<<node_grid, NODE_THREADS, 0, st>>>(na);
   }
-  k_clf_readout<<<num_mols, CH, 0, st>>>(nodeout, mol_off, h->g, pred);
+  k_clf_readout<false><<<num_mols, CH, 0, st>>>(nodeout, mol_off, h->g, pred);
   e = cudaGetLastError();
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "classifier forward: %s", cudaGetErrorString(e));
+  return BDIFF_OK;
+}
+
+int64_t bdiff_classifier_param_floats(const bdiff_classifier* h) { return h ? h->pfloats : 0; }
+
+int32_t bdiff_classifier_param_layout(bdiff_classifier* h, const char* name, int64_t* offset, int64_t* count) {
+  if (!h || !name || !offset || !count) return h ? h->fail(BDIFF_EINVAL, "bad argument") : BDIFF_EINVAL;
+  auto it = h->playout.find(name);
+  if (it == h->playout.end()) return h->fail(BDIFF_EINVAL, "unknown parameter name '%s'", name);
+  *offset = it->second.first;
+  *count = it->second.second;
+  return BDIFF_OK;
+}
+
+int32_t bdiff_classifier_train_forward(bdiff_classifier* h, void* stream, int32_t num_mols, const int32_t* mol_off_host,
+                                       const float* x, const float* one_hot, float* pred) {
+  if (!h) return BDIFF_EINVAL;
+  if (num_mols < 1 || !mol_off_host || !x || !one_hot || !pred) return h->fail(BDIFF_EINVAL, "bad argument");
+  std::vector<long long> pair_off;
+  if (const int rc = check_batch(h, num_mols, mol_off_host, pair_off)) return rc;
+  const int N = mol_off_host[num_mols], L = h->cfg.n_layers;
+  const long long E = pair_off[num_mols];
+  const long long ntiles = (E + CT - 1) / CT;
+  h->tape_valid = false;
+  ClfTape t{};
+  cudaError_t e = grow_buf(h->tape, h->tape_bytes, tape_carve(nullptr, L, N, num_mols, t));
+  if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "tape: %s", cudaGetErrorString(e));
+  tape_carve(static_cast<unsigned char*>(h->tape), L, N, num_mols, t);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t nc = (size_t)N * CH;
+  cudaMemcpyAsync(t.mol_off, mol_off_host, (size_t)(num_mols + 1) * 4, cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(t.pair_off, pair_off.data(), (size_t)(num_mols + 1) * 8, cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(t.x, x, (size_t)N * 3 * sizeof(float), cudaMemcpyDeviceToDevice, st);
+  cudaMemcpyAsync(t.oh, one_hot, (size_t)N * CIN * sizeof(float), cudaMemcpyDeviceToDevice, st);
+  cudaMemsetAsync(t.agg, 0, (size_t)L * nc * sizeof(float), st);    // every layer's agg: the edge kernel's red.add words
+
+  // the inference kernels' schedule; TAPE = true node / readout kernels keep what the reverse sweep reads
+  ClfNodeArgs na{};
+  na.one_hot = t.oh; na.nodeout = t.nodeout; na.N = N; na.L = L; na.node_attr = h->cfg.node_attr; na.g = h->g;
+  na.q = t.q; na.qs = t.qs;
+  const int node_grid = (N + NT - 1) / NT;
+  ClfEdgeArgs ea{};
+  ea.x = t.x; ea.mol_off = t.mol_off; ea.pair_off = t.pair_off; ea.B = num_mols; ea.E = E;
+  ea.ntiles = (int)ntiles; ea.attention = h->cfg.attention;
+  const int edge_grid = (int)std::min<long long>(ntiles, h->num_sms);
+  for (int l = -1; l < L; ++l) {
+    if (l >= 0) {
+      ea.w = h->layers[l];
+      ea.P = t.P + l * nc; ea.Q = t.Q + l * nc; ea.agg = t.agg + l * nc;
+      k_clf_edge<<<edge_grid, EDGE_THREADS, EDGE_SMEM, st>>>(ea);
+    }
+    na.layer = l;
+    na.h = l >= 0 ? t.h + l * nc : nullptr;
+    na.h_out = t.h + (l + 1) * nc;
+    if (l >= 0) {
+      na.cur = h->layers[l];
+      na.agg = t.agg + l * nc; na.v = t.v + l * nc; na.u = t.u + l * nc;
+    }
+    if (l + 1 < L) { na.nxt = h->layers[l + 1]; na.P = t.P + (l + 1) * nc; na.Q = t.Q + (l + 1) * nc; }
+    k_clf_node<true><<<node_grid, NODE_THREADS, 0, st>>>(na);
+  }
+  k_clf_readout<true><<<num_mols, CH, 0, st>>>(t.nodeout, t.mol_off, h->g, pred, t.s, t.w, t.ws);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "classifier training forward: %s", cudaGetErrorString(e));
+  h->tape_valid = true;
+  h->tape_weights_gen = h->weights_gen;
+  h->tape_B = num_mols; h->tape_N = N; h->tape_E = E;
+  return BDIFF_OK;
+}
+
+int32_t bdiff_classifier_train_backward(bdiff_classifier* h, void* stream, const float* d_pred, float* grad_flat) {
+  if (!h) return BDIFF_EINVAL;
+  if (!d_pred || !grad_flat) return h->fail(BDIFF_EINVAL, "bad argument");
+  if (!h->tape_valid) return h->fail(BDIFF_ESTATE, "no tape: run bdiff_classifier_train_forward first");
+  if (h->tape_weights_gen != h->weights_gen)
+    return h->fail(BDIFF_ESTATE, "the weights changed after the training forward: its tape is stale");
+  const int B = h->tape_B, N = h->tape_N, L = h->cfg.n_layers;
+  const long long E = h->tape_E, ntiles = (E + CT - 1) / CT;
+  ClfTape t{};
+  tape_carve(static_cast<unsigned char*>(h->tape), L, N, B, t);
+  ClfBwdScratch b{};
+  cudaError_t e = grow_buf(h->bws, h->bws_bytes, bws_carve(nullptr, N, B, E, b));
+  if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "backward scratch: %s", cudaGetErrorString(e));
+  bws_carve(static_cast<unsigned char*>(h->bws), N, B, E, b);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t nc = (size_t)N * CH;
+  const int in3 = 2 * CH + (h->cfg.node_attr ? CIN : 0);
+  auto G = [&](const std::string& name) { return grad_flat + h->playout.at(name).first; };
+  cudaMemsetAsync(grad_flat, 0, (size_t)h->pfloats * sizeof(float), st);     // the alignment gaps
+
+  // readout: graph_dec, the molecule sum, node_dec (EGNN.forward :415-419)
+  k_clf_bwd_readout<<<B, CH, 0, st>>>(d_pred, t.w, h->g, b.dWk, b.dS);
+  wgrad(st, b.part, d_pred, 1, t.ws, CH, 1, CH, B, G("graph_dec.2.weight"), CH, 0, G("graph_dec.2.bias"), 1);
+  wgrad(st, b.part, b.dWk, CH, t.s, CH, CH, CH, B, G("graph_dec.0.weight"), CH, 0, G("graph_dec.0.bias"), 1);
+  const int node_grid = (N + NT - 1) / NT;
+  ClfBwdDecArgs da{b.dS, t.q, t.mol_off, B, N, h->g, b.dY, b.dQd, b.dHa};
+  k_clf_bwd_nodedec<<<node_grid, NODE_THREADS, 0, st>>>(da);
+  wgrad(st, b.part, b.dY, CH, t.qs, CH, CH, CH, N, G("node_dec.2.weight"), CH, 0, G("node_dec.2.bias"), 1);
+  wgrad(st, b.part, b.dQd, CH, t.h + L * nc, CH, CH, CH, N, G("node_dec.0.weight"), CH, 0, G("node_dec.0.bias"), 1);
+
+  float *dHo = b.dHa, *dH = b.dHb;
+  ClfBwdEdgeArgs ea{};
+  ea.x = t.x; ea.dAgg = b.dAgg; ea.mol_off = t.mol_off; ea.pair_off = t.pair_off; ea.B = B; ea.E = E;
+  ea.ntiles = (int)ntiles; ea.attention = h->cfg.attention;
+  ea.A = b.A; ea.S = b.S; ea.DZ2 = b.DZ2; ea.DT = b.DT; ea.DZ1 = b.DZ1;
+  const int edge_grid = (int)std::min<long long>(ntiles, h->num_sms);
+  for (int l = L - 1; l >= 0; --l) {
+    const std::string p = "gcl_" + std::to_string(l) + ".";
+    const float* hl = t.h + l * nc;
+    // node_mlp (E_GCL.node_model :318-328)
+    ClfBwdNodeArgs nb{dHo, t.v + l * nc, N, h->layers[l], b.dV, dH, b.dAgg};
+    k_clf_bwd_node<<<node_grid, NODE_THREADS, 0, st>>>(nb);
+    wgrad(st, b.part, dHo, CH, t.u + l * nc, CH, CH, CH, N, G(p + "node_mlp.2.weight"), CH, 0, G(p + "node_mlp.2.bias"), 1);
+    wgrad(st, b.part, b.dV, CH, hl, CH, CH, CH, N, G(p + "node_mlp.0.weight"), in3, 0, G(p + "node_mlp.0.bias"), 1);
+    wgrad(st, b.part, b.dV, CH, t.agg + l * nc, CH, CH, CH, N, G(p + "node_mlp.0.weight"), in3, CH, nullptr, 1);
+    if (h->cfg.node_attr)
+      wgrad(st, b.part, b.dV, CH, t.oh, CIN, CH, CIN, N, G(p + "node_mlp.0.weight"), in3, 2 * CH, nullptr, 1);
+    // edge side (E_GCL.edge_model :306-316, the mask of E_GCL_mask.forward :357)
+    ea.P = t.P + l * nc; ea.Q = t.Q + l * nc; ea.w = h->layers[l]; ea.W2Ts = h->w2tbuf + (size_t)l * W2_BYTES;
+    k_clf_bwd_edge<<<edge_grid, EDGE_THREADS, BWD_EDGE_SMEM, st>>>(ea);
+    if (h->cfg.attention)
+      wgrad(st, b.part, b.DT, 1, b.S, CH, 1, CH, E, G(p + "att_mlp.0.weight"), CH, 0, G(p + "att_mlp.0.bias"), 1);
+    wgrad(st, b.part, b.DZ2, CH, b.A, CH, CH, CH, E, G(p + "edge_mlp.2.weight"), CH, 0, G(p + "edge_mlp.2.bias"), 1);
+    k_clf_bwd_pairs<<<N, CH, 0, st>>>(b.DZ1, t.x, t.mol_off, t.pair_off, B, b.dP, b.dQ, b.R);
+    float* w1 = G(p + "edge_mlp.0.weight");
+    wgrad(st, b.part, b.dP, CH, hl, CH, CH, CH, N, w1, 2 * CH + 1, 0, G(p + "edge_mlp.0.bias"), 1);
+    wgrad(st, b.part, b.dQ, CH, hl, CH, CH, CH, N, w1, 2 * CH + 1, CH, nullptr, 1);
+    wgrad(st, b.part, b.R, CH, nullptr, 0, CH, 0, N, nullptr, 0, 0, w1 + 2 * CH, 2 * CH + 1);
+    k_clf_bwd_dh_edge<<<node_grid, NODE_THREADS, 0, st>>>(b.dP, b.dQ, N, h->layers[l], dH);
+    std::swap(dHo, dH);
+  }
+  // embedding (EGNN.forward :407); h0 and x are data: no input gradient
+  wgrad(st, b.part, dHo, CH, t.oh, CIN, CH, CIN, N, G("embedding.weight"), CIN, 0, G("embedding.bias"), 1);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "classifier training backward: %s", cudaGetErrorString(e));
   return BDIFF_OK;
 }
 

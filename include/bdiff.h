@@ -312,6 +312,30 @@ BDIFF_API int32_t bdiff_classifier_set_weight(bdiff_classifier* h, void* stream,
 BDIFF_API int32_t bdiff_classifier_forward(bdiff_classifier* h, void* stream, int32_t num_mols, const int32_t* mol_off_host,
                                            const float* x, const float* one_hot, float* pred);
 
+/* ---- training pass of the EGNN property classifier -------------------------------------------------------------------
+ * Replaces: loss.backward() through EGNN.forward (src/__init__.py:368-419) in the train branch of
+ * train_with_property_classifier (:144-204): the L1 loss of pred against (label - mean) / mad, loss.backward(), then a
+ * torch optimiser step.
+ *
+ * Gradients travel as ONE flat fp32 buffer in a canonical layout: the reference tensors (set_weight's names and shapes,
+ * nn.Linear weights [out,in] row-major) in ascending name order, each starting at a multiple of 64 floats.
+ * bdiff_classifier_param_floats = length of such a buffer; bdiff_classifier_param_layout = {offset, count} of one tensor.
+ *
+ * bdiff_classifier_train_forward: same arguments and bit-identical pred as bdiff_classifier_forward, and keeps the tape
+ *   (per layer h, the edge_mlp.0 node halves P / Q, agg, node_mlp.0's pre-activation and SiLU; node_dec's and graph_dec's
+ *   pre-activations and the molecule sums; copies of x, one_hot and the offsets) in device memory owned by the handle.
+ *   One tape per handle: the next training forward replaces it.
+ * bdiff_classifier_train_backward: grad_flat <- d/dparams sum_k pred_k d_pred[k] for the tape of the last training
+ *   forward (overwritten, not accumulated into; x and one_hot get no gradient).  No atomics: bit-reproducible.
+ *   BDIFF_ESTATE without a tape or when set_weight ran after the training forward (the tape's weights are gone).
+ * Both on `stream`; the forward copies mol_off to the device, neither synchronises. */
+BDIFF_API int64_t bdiff_classifier_param_floats(const bdiff_classifier* h);
+BDIFF_API int32_t bdiff_classifier_param_layout(bdiff_classifier* h, const char* name, int64_t* offset, int64_t* count);
+BDIFF_API int32_t bdiff_classifier_train_forward(bdiff_classifier* h, void* stream, int32_t num_mols,
+                                                 const int32_t* mol_off_host, const float* x, const float* one_hot,
+                                                 float* pred);
+BDIFF_API int32_t bdiff_classifier_train_backward(bdiff_classifier* h, void* stream, const float* d_pred, float* grad_flat);
+
 #ifdef __cplusplus
 }
 #endif

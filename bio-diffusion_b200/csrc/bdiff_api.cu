@@ -215,6 +215,10 @@ int32_t bdiff_create(const bdiff_config* cfg, bdiff_handle** out) {
   if (cfg->num_h < 1 || cfg->num_context < 0 || cfg->num_h + 1 + cfg->num_context > 28) { g_create_error = "num_h + 1 + num_context must be in [2,28]"; return BDIFF_EINVAL; }
   if (cfg->num_layers < 1 || cfg->num_layers > 64) { g_create_error = "num_layers out of range"; return BDIFF_EINVAL; }
   if (cfg->mode != BDIFF_MODE_PARITY_FP32 && cfg->mode != BDIFF_MODE_TENSOR) { g_create_error = "unknown mode"; return BDIFF_EINVAL; }
+  if (cfg->mode == BDIFF_MODE_TENSOR && !tc_supported(cfg->e_hidden, cfg->xi_hidden)) {
+    g_create_error = "tensor mode supports (e_hidden, xi_hidden) in {(64,16), (16,8)} only";
+    return BDIFF_EINVAL;
+  }
   int dev_count = 0;
   if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count == 0) {
     g_create_error = "no CUDA device: libbdiff_sm90 has no CPU fallback";
@@ -272,12 +276,6 @@ int32_t bdiff_create(const bdiff_config* cfg, bdiff_handle** out) {
   }
   cudaError_t e = configure_kernels();
   if (e == cudaSuccess && cfg->mode == BDIFF_MODE_TENSOR) {
-    if (!tc_supported(d.Ed, d.Xd)) {
-      g_create_error = "tensor mode supports (e_hidden, xi_hidden) in {(64,16), (16,8)} only";
-      cudaFree(h->wbuf);
-      delete h;
-      return BDIFF_EINVAL;
-    }
     e = tc_layers_configure();
     h->tc_layer_bytes = tc_blob_bytes(d.Ed, d.Xd);
     h->tc_node_layer_bytes = tc_node_blob_bytes();
@@ -533,7 +531,8 @@ int32_t bdiff_plan_topology(bdiff_handle* h, void* stream, int32_t num_mols, int
     // reads node pairs <= ndep(j), whose time is l*PE + edep(ndep) + lag  <  (l+1)*PE + j.
     const int L = h->d.L, TE = (int)ntile128, TN = ntile32;
     const int PE = (TE + 1) / 2, PN = (TN + 1) / 2;
-    if (L > 63 || ntile128 >= (1 << 24) || ntile32 >= (1 << 24)) return h->fail(BDIFF_EINVAL, "problem too large for the tile scheduler");
+    // an item packs the layer into bits 24..29 (0..63, so up to the 64 layers bdiff_create accepts) and the pair into 0..23
+    if (L > 64 || ntile128 >= (1 << 24) || ntile32 >= (1 << 24)) return h->fail(BDIFF_EINVAL, "problem too large for the tile scheduler");
     auto node_pair_last_edge_pair = [&](int v) {          // last edge pair a node pair depends on (-1: none)
       int th = -1;
       for (int u = 2 * v; u < std::min(TN, 2 * v + 2); ++u) th = std::max(th, node_dep[2 * u + 1]);

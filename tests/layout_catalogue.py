@@ -3,7 +3,8 @@
 
 A molecule with `na` active atoms has na x na edges, row by row; edge tiles hold 128 edges in eight 16-row windows, node
 tiles 32 atoms.  `layout_paths` restates those tiling rules in plain Python (see test_gpu_tc_layouts.py for the paths).
-`_inputs` builds a case's seeded inputs: masked xh rows zero, coordinates centred per molecule, t and context per molecule.
+`_inputs` builds a case's seeded inputs: masked xh rows zero, coordinates centred per molecule, t and context per molecule,
+for the case's configuration or any other (test_gpu_configs.py).
 """
 from dataclasses import dataclass, field
 from typing import List, Tuple
@@ -163,9 +164,10 @@ def layout_paths(sizes, mask, config="qm9"):
     return paths
 
 
-def _inputs(c: Layout):
-    """Seeded inputs of a case: masked xh rows are zero, coordinates centred per molecule, t and context per molecule."""
-    ocfg = O.config_named(c.config)
+def _inputs(c: Layout, ocfg: O.OracleConfig = None):
+    """Seeded inputs of a case: masked xh rows are zero, coordinates centred per molecule, t and context per molecule.
+    `ocfg` gives the feature and context widths of another configuration than the case's own."""
+    ocfg = ocfg or O.config_named(c.config)
     g = torch.Generator().manual_seed(sum(map(ord, c.name)))
     b = len(c.sizes)
     bi = torch.repeat_interleave(torch.arange(b), torch.tensor(c.sizes))

@@ -122,8 +122,9 @@ def _d_out(c: Layout) -> torch.Tensor:
 
 
 def oracle_grads(sd, config, inputs, d_out, dtype=torch.float64):
-    """net_out and d sum(net_out * d_out) / d theta for every parameter, by torch.autograd through the oracle."""
-    ocfg = O.config_named(config)
+    """net_out and d sum(net_out * d_out) / d theta for every parameter, by torch.autograd through the oracle; `config`
+    is a shipped configuration's name or an OracleConfig."""
+    ocfg = O.config_named(config) if isinstance(config, str) else config
     leaves = {k: v.detach().to(dtype).clone().requires_grad_(True) for k, v in sd.items()}
     out = O.denoiser_forward(leaves, ocfg, *inputs, dtype=dtype, guard_empty=True)
     grads = torch.autograd.grad(out, list(leaves.values()), d_out.to(dtype), allow_unused=True)

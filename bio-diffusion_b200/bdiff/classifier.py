@@ -56,6 +56,21 @@ def classifier_parameter_shapes(n_layers: int, attention: bool, node_attr: bool,
     return out
 
 
+def predict_inputs(x: torch.Tensor, one_hot: torch.Tensor, num_nodes) -> torch.Tensor:
+    """Validates the packed batch of `PropertyClassifier.predict` on the host; returns num_nodes as int64 [B] on the CPU."""
+    nn_ = torch.as_tensor(num_nodes).reshape(-1).to("cpu", torch.int64)
+    n = int(x.shape[0])
+    if x.dim() != 2 or x.shape[1] != 3:
+        raise ValueError(f"x must be [N, 3], got {tuple(x.shape)}")
+    if one_hot.dim() != 2 or one_hot.shape != (n, IN_NODE_NF):
+        raise ValueError(f"one_hot must be [N, {IN_NODE_NF}] = [{n}, {IN_NODE_NF}], got {tuple(one_hot.shape)}")
+    if nn_.numel() < 1 or int(nn_.sum()) != n or bool((nn_ < 1).any()):
+        raise ValueError("num_nodes must be positive and sum to the number of atoms")
+    if int(nn_.max()) > MAX_ATOMS:
+        raise ValueError(f"a molecule has {int(nn_.max())} atoms: the classifier takes at most {MAX_ATOMS}")
+    return nn_
+
+
 class _ClassifierTrainFn(torch.autograd.Function):
     """pred = classifier(params; x, one_hot) with the library's tape; backward = bdiff_classifier_train_backward."""
 
@@ -184,16 +199,7 @@ class PropertyClassifier(nn.Module):
         """pred [B] (normalised property) of packed molecules: x [N, 3], one_hot [N, 5] (the sampler's out[:, :3] and
         out[:, 3:8]), num_nodes [B] with 1 <= n <= 128 summing to N.  Under autograd with trainable parameters the
         result carries a grad_fn (the training pass; its values are bit-identical to the inference kernels')."""
-        nn_ = torch.as_tensor(num_nodes).reshape(-1).to("cpu", torch.int64)
-        n = int(x.shape[0])
-        if x.dim() != 2 or x.shape[1] != 3:
-            raise ValueError(f"x must be [N, 3], got {tuple(x.shape)}")
-        if one_hot.dim() != 2 or one_hot.shape != (n, IN_NODE_NF):
-            raise ValueError(f"one_hot must be [N, {IN_NODE_NF}] = [{n}, {IN_NODE_NF}], got {tuple(one_hot.shape)}")
-        if nn_.numel() < 1 or int(nn_.sum()) != n or bool((nn_ < 1).any()):
-            raise ValueError("num_nodes must be positive and sum to the number of atoms")
-        if int(nn_.max()) > MAX_ATOMS:
-            raise ValueError(f"a molecule has {int(nn_.max())} atoms: the classifier takes at most {MAX_ATOMS}")
+        nn_ = predict_inputs(x, one_hot, num_nodes)
         if not x.is_cuda:
             raise _lib.BdiffError("PropertyClassifier runs on CUDA tensors only (no CPU fallback)")
         off = torch.zeros(int(nn_.numel()) + 1, dtype=torch.int32)

@@ -288,7 +288,14 @@ class GCDMSampler:
         if cfg.include_charges:
             raise NotImplementedError("mol_gen_optimize stacks [x | one-hot] only: needs include_charges=False")
         check_frames(cfg.num_timesteps if num_timesteps is None else int(num_timesteps), return_frames)
-        dev = self._device()
+        z = self._optimize_latent(cfg, samples, num_nodes, self._device(), node_mask)
+        return self.sample(num_nodes, context, num_timesteps, node_mask, noise, z_init=z, return_frames=return_frames)
+
+    @staticmethod
+    def _optimize_latent(cfg, samples, num_nodes: torch.Tensor, dev: torch.device,
+                         node_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The starting latent of `optimize`: the molecules normalised into z [N, 3+F] on `dev`, after the reference's
+        mean-zero assertion, which sums the positions of the whole batch."""
         x = torch.vstack([s[0] for s in samples]).to(dev, torch.float32)
         hc = torch.vstack([s[1] for s in samples]).to(dev, torch.float32)
         n = x.shape[0]
@@ -302,7 +309,7 @@ class GCDMSampler:
         err = z[:, :3].sum(dim=0).abs().max().item()                          # the reference sums over the WHOLE batch
         if err / (largest + 1e-10) >= 1e-2:
             raise AssertionError(f"Mean is not zero, as relative_error {err / (largest + 1e-10)}")
-        return self.sample(num_nodes, context, num_timesteps, node_mask, noise, z_init=z, return_frames=return_frames)
+        return z
 
     @staticmethod
     def _inpaint_inputs(cfg, molecule, node_mask_fixed, context):

@@ -21,6 +21,26 @@ def _allowed_mask(atom_decoder: Sequence[str], allowed_bonds: Dict[str, Union[in
     return out
 
 
+def _check_batch(positions: torch.Tensor, atom_types: torch.Tensor, num_nodes: torch.Tensor, a: int) -> torch.Tensor:
+    """positions [N,3], atom_types [N] in [0, a), num_nodes [B] >= 0 summing to N; returns num_nodes int64 on the host."""
+    nn = num_nodes.detach().to(torch.int64).cpu()
+    n = int(positions.shape[0])
+    if positions.shape != (n, 3) or atom_types.shape != (n,) or int(nn.sum()) != n or (nn < 0).any():
+        raise ValueError("positions [N,3], atom_types [N] and num_nodes (summing to N) expected")
+    if n and (int(atom_types.min()) < 0 or int(atom_types.max()) >= a):
+        raise ValueError("atom type outside the decoder")
+    return nn
+
+
+def stability_inputs(positions: torch.Tensor, atom_types: torch.Tensor, num_nodes: torch.Tensor, dataset_info: dict,
+                     allowed_bonds: Dict[str, Union[int, Sequence[int]]]) -> torch.Tensor:
+    """The argument checks of check_molecular_stability_batch that do not depend on the device; returns num_nodes int64
+    on the host."""
+    dec = list(dataset_info["atom_decoder"])
+    _allowed_mask(dec, allowed_bonds)
+    return _check_batch(positions, atom_types, num_nodes, len(dec))
+
+
 def check_molecular_stability_batch(positions: torch.Tensor, atom_types: torch.Tensor, num_nodes: torch.Tensor,
                                     dataset_info: dict, allowed_bonds: Dict[str, Union[int, Sequence[int]]],
                                     margins: Tuple[float, float, float] = (10.0, 5.0, 3.0),
@@ -40,12 +60,8 @@ def check_molecular_stability_batch(positions: torch.Tensor, atom_types: torch.T
     mask = torch.from_numpy(_allowed_mask(dec, allowed_bonds).view(np.int32)).to(dev)
     x = positions.detach().to(torch.float32).contiguous()
     t = atom_types.detach().to(torch.int32).contiguous()
-    nn = num_nodes.detach().to(torch.int64).cpu()
+    nn = _check_batch(x, t, num_nodes, a)
     n = int(x.shape[0])
-    if x.shape != (n, 3) or t.shape != (n,) or int(nn.sum()) != n or (nn < 0).any():
-        raise ValueError("positions [N,3], atom_types [N] and num_nodes (summing to N) expected")
-    if n and (int(t.min()) < 0 or int(t.max()) >= a):
-        raise ValueError("atom type outside the decoder")
     b = int(nn.numel())
     off = torch.zeros(b + 1, dtype=torch.int32)
     off[1:] = torch.cumsum(nn, 0).to(torch.int32)

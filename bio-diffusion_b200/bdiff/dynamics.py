@@ -211,22 +211,12 @@ class GCPNetDynamicsB200(nn.Module):
         lib = _lib.load()
         self.sync_weights()
         _, n, _ = self.plan(batch_index, mask, num_mols)
-        xh_c = xh.detach().to(torch.float32).contiguous()
-        t_c = t.detach().to(torch.float32).reshape(-1).contiguous()
-        if t_c.numel() == 1:
-            t_c = t_c.expand(n).contiguous()
-        if xh_c.shape != (n, 3 + self.cfg.num_h) or t_c.shape[0] != n:
-            raise ValueError(f"xh must be [{n},{3 + self.cfg.num_h}] and t [{n},1]")
-        ctx_ptr = None
-        if self.cfg.num_context:
-            if context is None:
-                raise ValueError("this configuration is property-conditional: batch.props_context is required")
-            ctx_c = context.detach().to(torch.float32).reshape(n, self.cfg.num_context).contiguous()
-            ctx_ptr = C.c_void_p(ctx_c.data_ptr())
+        xh_c, t_c, ctx_c = self._inputs(n, xh, t, context)
         out = torch.empty_like(xh_c)
         _lib.check(self._handle, lib.bdiff_denoise_forward(
-            self._handle, self._stream(), C.c_void_p(xh_c.data_ptr()), C.c_void_p(t_c.data_ptr()), ctx_ptr,
-            C.c_void_p(out.data_ptr())), "bdiff_denoise_forward")
+            self._handle, self._stream(), C.c_void_p(xh_c.data_ptr()), C.c_void_p(t_c.data_ptr()),
+            C.c_void_p(ctx_c.data_ptr()) if ctx_c is not None else None, C.c_void_p(out.data_ptr())),
+            "bdiff_denoise_forward")
         return out
 
     def wants_grad(self) -> bool:
@@ -335,17 +325,13 @@ class GCPNetDynamicsB200(nn.Module):
         lib = _lib.load()
         self.sync_weights()
         _, n, _ = self.plan(batch_index, mask, num_mols)
-        xh_c = xh.detach().to(torch.float32).contiguous()
-        t_c = t.detach().to(torch.float32).reshape(-1).contiguous()
-        ctx_ptr = None
-        if self.cfg.num_context:
-            ctx_c = context.detach().to(torch.float32).reshape(n, self.cfg.num_context).contiguous()
-            ctx_ptr = C.c_void_p(ctx_c.data_ptr())
+        xh_c, t_c, ctx_c = self._inputs(n, xh, t, context)
         out = torch.empty_like(xh_c)
         ms = (C.c_float * 8)()
         _lib.check(self._handle, lib.bdiff_profile_forward(
-            self._handle, self._stream(), C.c_void_p(xh_c.data_ptr()), C.c_void_p(t_c.data_ptr()), ctx_ptr,
-            C.c_void_p(out.data_ptr()), ms), "bdiff_profile_forward")
+            self._handle, self._stream(), C.c_void_p(xh_c.data_ptr()), C.c_void_p(t_c.data_ptr()),
+            C.c_void_p(ctx_c.data_ptr()) if ctx_c is not None else None, C.c_void_p(out.data_ptr()), ms),
+            "bdiff_profile_forward")
         names = ("prep", "edge_embed", "node_embed", "edge_message", "node_update", "finalize", "total")
         prof = {k: float(ms[i]) for i, k in enumerate(names)}
         if ms[7] < 0:       # tensor mode default: all layers ran as ONE persistent kernel (k_layers_tc)

@@ -6,9 +6,9 @@ one reverse step = two torch.randn draws (same order as the reference: randn(N,3
 C-ABI call (bdiff_reverse_step: 4+2L+2 kernels) + a device counter bump, captured ONCE in a CUDA graph and
 replayed T times — no host synchronisation inside the chain.
 
-inpaint (variational_diffusion.py:1580-1789, RePaint) replays two such graphs in the order of the RePaint schedule: the
-denoise op (4 draws, the reverse step, bdiff_repaint_combine, frame write, op counter bump) and the jump back (2 draws,
-bdiff_renoise, jump counter bump).  Every per-op coefficient is read on the device at the counters.
+inpaint (variational_diffusion.py:1580-1789, RePaint) runs the same chain with two bodies replayed in the order of the
+RePaint schedule: the denoise op (4 draws, the reverse step, bdiff_repaint_combine, frame write, op counter bump) and the
+jump back (2 draws, bdiff_renoise, jump counter bump).  Every per-op coefficient is read on the device at the counters.
 """
 from __future__ import annotations
 
@@ -26,18 +26,20 @@ from .schedule import (chain_frame_slots, check_frames, check_repaint, decode_co
 NoiseFn = Callable[[Tuple[int, int]], torch.Tensor]
 
 
+def _ptr(t: Optional[torch.Tensor]) -> Optional[C.c_void_p]:
+    return None if t is None else C.c_void_p(t.data_ptr())
+
+
 class GCDMSampler:
     def __init__(self, dynamics: GCPNetDynamicsB200, use_cuda_graph: bool = True):
         self.net = dynamics
         self.cfg = dynamics.cfg
         self.use_cuda_graph = use_cuda_graph
         self.gamma = gamma_table(self.cfg.num_timesteps, self.cfg.noise_precision, self.cfg.noise_schedule)
+        self._static = None          # every device buffer the chain's graphs read or write (see _statics)
+        self._graphs = None          # the captured bodies of the chain on these statics, and their key
         self._graph_key = None
-        self._graph = None
-        self._static = None
-        self._ip = None              # inpaint: statics, and the op / jump graphs with their key
-        self._ip_graphs = None
-        self._ip_graph_key = None
+        self._topo = None            # (batch_index, mask) of the last plan
         self.kernel_launches = 0     # libbdiff kernels launched (or replayed from the graph) by sample() / inpaint()
         self.last_moments = None     # [T, 4] per-step (mean|x|, max|x|, mean h, mean|h|) of z when sample(record_moments=True)
 
@@ -45,39 +47,167 @@ class GCDMSampler:
     def _device(self) -> torch.device:
         return next(self.net.parameters()).device
 
-    def _statics(self, n: int, steps: int, dev: torch.device):
-        key = (n, steps, dev)
+    def _statics(self, n: int, steps: int, repaint: Optional[Tuple[int, int]], frames: int, moments: bool,
+                 dev: torch.device):
+        """The chain's device buffers and tables, cached by shape and chain kind (plain, or RePaint with (r, j)).
+        Building new statics drops the graphs captured on the old ones."""
+        key = (n, steps, repaint, frames, moments, dev)
         if self._static is not None and self._static["key"] == key:
             return self._static
-        f = self.cfg.num_h
-        st = dict(key=key,
-                  z=torch.zeros((n, 3 + f), device=dev), nx=torch.zeros((n, 3), device=dev),
-                  nh=torch.zeros((n, f), device=dev), step=torch.zeros((), dtype=torch.int32, device=dev),
-                  coef=step_coefficient_table(self.gamma, steps).to(dev),
-                  dec=decode_coefficients(self.gamma).to(dev), xh=torch.zeros((n, 3 + f), device=dev))
+        f, c = self.cfg.num_h, self.cfg.num_context
+
+        def zeros(*shape, dtype=torch.float32):
+            return torch.zeros(shape, dtype=dtype, device=dev)
+
+        if repaint is None:
+            prog = dict(rev=step_coefficient_table(self.gamma, steps), slot=chain_frame_slots(steps, frames),
+                        jump_after=[False] * steps, num_jumps=0)
+        else:
+            prog = repaint_program(self.gamma, *repaint, steps, frames)
+        st = dict(key=key, repaint=repaint, schedule=prog["jump_after"], num_jumps=prog["num_jumps"],
+                  z=zeros(n, 3 + f), xh=zeros(n, 3 + f), nx=zeros(n, 3), nh=zeros(n, f),
+                  step=zeros(dtype=torch.int32), coef=prog["rev"].to(dev), dec=decode_coefficients(self.gamma).to(dev),
+                  ctx=zeros(n, c) if c else None, mf=zeros(n, 1), slot=prog["slot"].to(dev),
+                  frames=zeros(frames + 1, n, 3 + f) if frames > 1 else None,
+                  moments=zeros(steps, 4) if moments else None)
+        if repaint is not None:
+            st.update(kx=zeros(n, 3), kh=zeros(n, f), jstep=zeros(dtype=torch.int32), known=prog["known"].to(dev),
+                      jump=prog["jump"].to(dev), xh0=zeros(n, 3 + f), fixed=zeros(n, dtype=torch.uint8))
         self._static = st
-        self._graph = None
+        self._graphs = None
         self._graph_key = None
         return st
 
-    def _reverse_step(self, st, ctx_ptr):
-        lib = _lib.load()
-        h = self.net._handle
-        _lib.check(h, lib.bdiff_reverse_step(h, self.net._stream(), C.c_void_p(st["z"].data_ptr()), ctx_ptr,
-                                             C.c_void_p(st["nx"].data_ptr()), C.c_void_p(st["nh"].data_ptr()),
-                                             C.c_void_p(st["coef"].data_ptr()), C.c_void_p(st["step"].data_ptr())),
-                   "bdiff_reverse_step")
+    def _prepare(self, batch_index: torch.Tensor, mask: torch.Tensor, b: int, context: Optional[torch.Tensor],
+                 steps: int, repaint: Optional[Tuple[int, int]] = None, frames: int = 1, moments: bool = False):
+        """What every chain does before its first draw: weights, plan and statics for (batch_index, mask) on the
+        denoiser's device, and the per-atom context written into the statics.  Returns (statics, batch_index, mask)."""
+        dev = batch_index.device
+        if dev.type != "cuda":
+            raise _lib.BdiffError("GCDMSampler needs the denoiser on a CUDA device (no CPU fallback)")
+        if self.cfg.num_context and context is None:
+            raise ValueError("property-conditional configuration: `context` [B,C] is required")
+        self.net.sync_weights()
+        # the plan is keyed on tensor identity: reuse the tensors of the previous call when the topology repeats
+        if self._topo is not None:
+            pbi, pmask = self._topo
+            if pbi.shape == batch_index.shape and torch.equal(pbi, batch_index) and torch.equal(pmask, mask):
+                batch_index, mask = pbi, pmask
+        self.net.plan(batch_index, mask, b)
+        self._topo = (batch_index, mask)
+        st = self._statics(int(batch_index.shape[0]), steps, repaint, frames, moments, dev)
+        st["mf"].copy_(mask.float().unsqueeze(-1))
+        if st["ctx"] is not None:
+            st["ctx"].copy_(context.to(dev, torch.float32)[batch_index] * st["mf"])
+        return st, batch_index, mask
 
-    def _write_frame(self, frames: torch.Tensor, slots: torch.Tensor, counter: torch.Tensor, z: torch.Tensor,
-                     mf: torch.Tensor) -> None:
-        """frames[slots[counter]] = unnormalize_z(z) (variational_diffusion.py:762-792, 1353-1360), all on the device
+    @staticmethod
+    def _draw(noise: Optional[NoiseFn], *bufs: torch.Tensor) -> None:
+        """Fills each buffer in turn with N(0, I) draws: the device generator's, or `noise(shape)`'s when injected."""
+        for buf in bufs:
+            if noise is None:
+                torch.randn(buf.shape, device=buf.device, out=buf)
+            else:
+                buf.copy_(noise(tuple(buf.shape)))
+
+    def _reverse_step(self, z, ctx, nx, nh, coef, step) -> None:
+        h = self.net._handle
+        _lib.check(h, _lib.load().bdiff_reverse_step(h, self.net._stream(), _ptr(z), _ptr(ctx), _ptr(nx), _ptr(nh),
+                                                     _ptr(coef), _ptr(step)), "bdiff_reverse_step")
+
+    def _write_frame(self, st) -> None:
+        """frames[slot[step]] = unnormalize_z(z) (variational_diffusion.py:762-792, 1353-1360), all on the device
         so that it can sit in a captured graph; slot `return_frames` is the dummy row of ops that write no frame."""
         cfg = self.cfg
         a = cfg.num_atom_types
+        z, mf = st["z"], st["mf"]
         parts = [z[:, :3] * cfg.norm_values[0], (z[:, 3:3 + a] * cfg.norm_values[1] + cfg.norm_biases[1]) * mf]
         if cfg.include_charges:
             parts.append((z[:, 3 + a:] * cfg.norm_values[2] + cfg.norm_biases[2]) * mf)
-        frames.index_copy_(0, slots.index_select(0, counter.long().view(1)), torch.cat(parts, dim=-1).unsqueeze(0))
+        st["frames"].index_copy_(0, st["slot"].index_select(0, st["step"].long().view(1)),
+                                 torch.cat(parts, dim=-1).unsqueeze(0))
+
+    def _op(self, st, noise: Optional[NoiseFn]) -> None:
+        """One reverse step of the chain at the device counter: a `sample` step, or RePaint's denoise op, which draws the
+        known part's noise first (:1661-1667) and then combines the step's z_unknown (:1670-1679) with it."""
+        h = self.net._handle
+        if st["repaint"]:
+            self._draw(noise, st["kx"], st["kh"])
+        self._draw(noise, st["nx"], st["nh"])
+        self._reverse_step(st["z"], st["ctx"], st["nx"], st["nh"], st["coef"], st["step"])
+        if st["repaint"]:
+            _lib.check(h, _lib.load().bdiff_repaint_combine(h, self.net._stream(), _ptr(st["z"]), _ptr(st["xh0"]),
+                                                            _ptr(st["fixed"]), _ptr(st["kx"]), _ptr(st["kh"]),
+                                                            _ptr(st["known"]), _ptr(st["step"])), "bdiff_repaint_combine")
+        if st["moments"] is not None:
+            # diagnostics only (tests): moments of the latent after this step, written at row `step` on the device
+            zx, zh = st["z"][:, :3], st["z"][:, 3:]
+            m = torch.stack((zx.abs().mean(), zx.abs().max(), zh.mean(), zh.abs().mean())).view(1, 4)
+            st["moments"].index_copy_(0, st["step"].long().view(1), m)
+        if st["frames"] is not None:
+            self._write_frame(st)
+        st["step"].add_(1)
+
+    def _jump(self, st, noise: Optional[NoiseFn]) -> None:
+        """RePaint's jump back from s to t = s + jump_length (:1730-1749) at the jump counter."""
+        h = self.net._handle
+        self._draw(noise, st["nx"], st["nh"])
+        _lib.check(h, _lib.load().bdiff_renoise(h, self.net._stream(), _ptr(st["z"]), _ptr(st["nx"]), _ptr(st["nh"]),
+                                                _ptr(st["jump"]), _ptr(st["jstep"])), "bdiff_renoise")
+        st["jstep"].add_(1)
+
+    def _chain(self, st, noise: Optional[NoiseFn], batch_index: torch.Tensor, mask: torch.Tensor, b: int,
+               z_init: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Runs the chain on prepared statics from z_T (or from `z_init`) and decodes z_0: the output of sample /
+        inpaint, with the frames in front when the statics have them."""
+        lib = _lib.load()
+        h = self.net._handle
+        if z_init is None:
+            # z_T ~ N(0, I) on the zero-CoG subspace (variational_diffusion.py:1322-1328, 1635-1640)
+            self._draw(noise, st["nx"], st["nh"])
+            _lib.check(h, lib.bdiff_center_noise(h, self.net._stream(), _ptr(st["nx"]), _ptr(st["nh"]), _ptr(st["z"])),
+                       "bdiff_center_noise")
+        else:
+            st["z"].copy_(z_init)
+        for name in ("step", "jstep", "frames", "moments"):
+            if st.get(name) is not None:
+                st[name].zero_()
+
+        bodies = [lambda: self._op(st, noise)]
+        if st["num_jumps"]:
+            bodies.append(lambda: self._jump(st, noise))
+        if self.use_cuda_graph and noise is None:
+            # a captured graph bakes in raw pointers: of the statics, and of the library's weights and plan / workspace
+            # buffers, which move when a larger topology was planned in between (every bdiff_plan_topology bumps the
+            # plan epoch).  The key therefore holds no address of a tensor made per call.
+            key = (st["key"], self.net._plan_key, self.net._plan_epoch, self.net._weights_key)
+            if self._graph_key != key:
+                self._graphs = []
+                for body in bodies:
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g):
+                        body()
+                    self._graphs.append(g)
+                self._graph_key = key
+            bodies = [g.replay for g in self._graphs]
+        for jump in st["schedule"]:
+            bodies[0]()
+            if jump:
+                bodies[1]()
+
+        # one forward = prep, node_frames, edge_embed, node_embed, L x (edge_message, node_update), finalize; an op adds
+        # k_step (and k_repaint_combine), a jump k_step, the decode k_step
+        per_op = self.net.kernels_per_forward + 1 + (1 if st["repaint"] else 0)
+        self.kernel_launches += ((1 if z_init is None else 0) + len(st["schedule"]) * per_op + st["num_jumps"]
+                                 + self.net.kernels_per_forward + 1)
+        # p(x, h | z_0) (variational_diffusion.py:1378-1387, 840-907), then the CoG fix when no frames are returned
+        self._draw(noise, st["nx"], st["nh"])
+        _lib.check(h, lib.bdiff_decode_z0(h, self.net._stream(), _ptr(st["z"]), _ptr(st["ctx"]), _ptr(st["nx"]),
+                                          _ptr(st["nh"]), _ptr(st["dec"]), _ptr(st["xh"])), "bdiff_decode_z0")
+        out = self._finish(st["xh"], batch_index, mask, b, cog_fix=st["frames"] is None)
+        if st["frames"] is not None:        # out[0] <- the molecules (:1404-1410, 1780-1786); the last row is the dummy
+            out = torch.cat((out.unsqueeze(0), st["frames"][1:-1]), dim=0)
+        return out
 
     def _finish(self, xh: torch.Tensor, batch_index: torch.Tensor, mask: torch.Tensor, b: int, cog_fix: bool):
         """Unnormalise and discretise p(x, h | z_0) (variational_diffusion.py:892-907), check the chain, CoG fix."""
@@ -121,123 +251,20 @@ class GCDMSampler:
         return_frames = F > 1, out is [F, N, 3+A(+1)]: frame k is the unnormalised latent after the step that lands on
         s = k*T/F, frame 0 the decoded molecules (no CoG drift correction, as in the reference).
         """
-        cfg = self.cfg
-        steps = cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
+        steps = self.cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
         check_frames(steps, return_frames)
         dev = self._device()
-        if dev.type != "cuda":
-            raise _lib.BdiffError("GCDMSampler needs the denoiser on a CUDA device (no CPU fallback)")
         num_nodes = num_nodes.to(dev, non_blocking=True)
         b = int(num_nodes.shape[0])
         batch_index = torch.repeat_interleave(torch.arange(b, device=dev), num_nodes)
         n = int(batch_index.shape[0])
         mask = torch.ones(n, dtype=torch.bool, device=dev) if node_mask is None else node_mask.to(dev)
-        ctx = None
-        ctx_ptr = None
-        if cfg.num_context:
-            if context is None:
-                raise ValueError("property-conditional configuration: `context` [B,C] is required")
-            ctx = (context.to(dev, torch.float32)[batch_index] * mask.float().unsqueeze(-1)).contiguous()
-            ctx_ptr = C.c_void_p(ctx.data_ptr())
-        self.net.sync_weights()
-        # the plan is keyed on tensor identity: reuse the tensors of the previous call when the topology repeats
-        if self._static is not None and self._static.get("topo") is not None:
-            pbi, pmask = self._static["topo"]
-            if pbi.shape == batch_index.shape and torch.equal(pbi, batch_index) and torch.equal(pmask, mask):
-                batch_index, mask = pbi, pmask
-        self.net.plan(batch_index, mask, b)
-        st = self._statics(n, steps, dev)
-        st["topo"] = (batch_index, mask)
-        lib = _lib.load()
-        h = self.net._handle
-        f = cfg.num_h
-
-        def draw(buf_x, buf_h):
-            if noise is None:
-                torch.randn((n, 3), device=dev, out=buf_x)
-                torch.randn((n, f), device=dev, out=buf_h)
-            else:
-                buf_x.copy_(noise((n, 3)))
-                buf_h.copy_(noise((n, f)))
-
-        if z_init is None:
-            # z_T ~ N(0, I) on the zero-CoG subspace (variational_diffusion.py:1322-1328)
-            draw(st["nx"], st["nh"])
-            _lib.check(h, lib.bdiff_center_noise(h, self.net._stream(), C.c_void_p(st["nx"].data_ptr()),
-                                                 C.c_void_p(st["nh"].data_ptr()), C.c_void_p(st["z"].data_ptr())),
-                       "bdiff_center_noise")
-        else:
-            if tuple(z_init.shape) != (n, 3 + f):
-                raise ValueError(f"z_init must be [{n}, {3 + f}]")
-            st["z"].copy_(z_init.to(dev, torch.float32))
-        st["step"].zero_()
-
-        moments = torch.zeros((steps, 4), device=dev) if record_moments else None
-
-        def record():
-            # diagnostics only (tests): moments of the latent after this step, written at row `step` on the device
-            zx, zh = st["z"][:, :3], st["z"][:, 3:]
-            m = torch.stack((zx.abs().mean(), zx.abs().max(), zh.mean(), zh.abs().mean())).view(1, 4)
-            moments.index_copy_(0, st["step"].long().view(1), m)
-
-        frames = None
-        if return_frames > 1:
-            fkey = ("frames", return_frames)
-            if fkey not in st:
-                st[fkey] = (torch.zeros((return_frames + 1, n, 3 + f), device=dev),
-                            chain_frame_slots(steps, return_frames).to(dev), torch.zeros((n, 1), device=dev))
-            frames, slots, mf_frames = st[fkey]
-            frames.zero_()
-            mf_frames.copy_(mask.float().unsqueeze(-1))
-
-        graph_ok = self.use_cuda_graph and noise is None
-        if graph_ok:
-            # the captured graph bakes in raw pointers of the library's plan / workspace buffers, which move when a larger
-            # topology was planned in between: the plan epoch (bumped by every bdiff_plan_topology) is part of the key
-            gkey = (st["key"], self.net._plan_key, self.net._plan_epoch, self.net._weights_key,
-                    ctx.data_ptr() if ctx is not None else 0, moments.data_ptr() if record_moments else 0)
-            if return_frames > 1:
-                gkey = gkey + (frames.data_ptr(),)
-            if self._graph is None or self._graph_key != gkey:
-                torch.cuda.current_stream().synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    draw(st["nx"], st["nh"])
-                    self._reverse_step(st, ctx_ptr)
-                    if record_moments:
-                        record()
-                    if return_frames > 1:
-                        self._write_frame(frames, slots, st["step"], st["z"], mf_frames)
-                    st["step"].add_(1)
-                self._graph, self._graph_key = g, gkey
-                self._ctx_keep = ctx
-            for _ in range(steps):
-                self._graph.replay()
-        else:
-            for _ in range(steps):
-                draw(st["nx"], st["nh"])
-                self._reverse_step(st, ctx_ptr)
-                if record_moments:
-                    record()
-                if return_frames > 1:
-                    self._write_frame(frames, slots, st["step"], st["z"], mf_frames)
-                st["step"].add_(1)
-        self.last_moments = moments
-
-        # one forward = prep, node_frames, edge_embed, node_embed, L x (edge_message, node_update), finalize
-        per_forward = self.net.kernels_per_forward
-        self.kernel_launches += 1 + steps * (per_forward + 1) + (per_forward + 1)
-        # p(x, h | z_0)  (variational_diffusion.py:1378-1387, 840-907)
-        z0 = st["z"].clone() if return_z0 else None
-        draw(st["nx"], st["nh"])
-        _lib.check(h, lib.bdiff_decode_z0(h, self.net._stream(), C.c_void_p(st["z"].data_ptr()), ctx_ptr,
-                                          C.c_void_p(st["nx"].data_ptr()), C.c_void_p(st["nh"].data_ptr()),
-                                          C.c_void_p(st["dec"].data_ptr()), C.c_void_p(st["xh"].data_ptr())),
-                   "bdiff_decode_z0")
-        out = self._finish(st["xh"], batch_index, mask, b, cog_fix=return_frames == 1)
-        if return_frames > 1:
-            out = torch.cat((out.unsqueeze(0), frames[1:return_frames]), dim=0)    # out[0] <- the molecules (:1404-1410)
-        return (out, batch_index, mask, z0) if return_z0 else (out, batch_index, mask)
+        st, batch_index, mask = self._prepare(batch_index, mask, b, context, steps, None, return_frames, record_moments)
+        if z_init is not None and tuple(z_init.shape) != (n, 3 + self.cfg.num_h):
+            raise ValueError(f"z_init must be [{n}, {3 + self.cfg.num_h}]")
+        out = self._chain(st, noise, batch_index, mask, b, z_init)
+        self.last_moments = st["moments"].clone() if record_moments else None
+        return (out, batch_index, mask, st["z"].clone()) if return_z0 else (out, batch_index, mask)
 
     def nan_guard_count(self, reset: bool = False) -> int:
         """Denoiser forwards in which the NaN guard of gcpnet.py:1214-1216 fired since the workspace was (re)planned."""
@@ -256,25 +283,15 @@ class GCDMSampler:
         dev = z.device
         self.net.sync_weights()
         self.net.plan(batch_index, mask, num_mols)
-        lib = _lib.load()
-        h = self.net._handle
         coef = step_coefficient_table(self.gamma, steps).to(dev)
         idx = torch.tensor(row, dtype=torch.int32, device=dev)
         zz = z.detach().to(torch.float32).clone().contiguous()
-        nx = noise_x.to(torch.float32).contiguous()
-        nh = noise_h.to(torch.float32).contiguous()
-        ctx_ptr = None
-        if self.cfg.num_context:
-            ctx = context.to(torch.float32).contiguous()
-            ctx_ptr = C.c_void_p(ctx.data_ptr())
-        _lib.check(h, lib.bdiff_reverse_step(h, self.net._stream(), C.c_void_p(zz.data_ptr()), ctx_ptr,
-                                             C.c_void_p(nx.data_ptr()), C.c_void_p(nh.data_ptr()),
-                                             C.c_void_p(coef.data_ptr()), C.c_void_p(idx.data_ptr())),
-                   "bdiff_reverse_step")
+        ctx = context.to(torch.float32).contiguous() if self.cfg.num_context else None
+        self._reverse_step(zz, ctx, noise_x.to(torch.float32).contiguous(), noise_h.to(torch.float32).contiguous(),
+                           coef, idx)
         torch.cuda.current_stream().synchronize()
         return zz
 
-    @torch.inference_mode()
     @torch.inference_mode()
     def optimize(self, samples, num_nodes: torch.Tensor, context: Optional[torch.Tensor] = None,
                  num_timesteps: Optional[int] = None, node_mask: Optional[torch.Tensor] = None,
@@ -348,27 +365,6 @@ class GCDMSampler:
             raise ValueError("`context` given to a configuration without conditioning")
         return num_nodes, batch_index, parts, node_mask_fixed.bool(), context
 
-    def _inpaint_statics(self, n: int, steps: int, r: int, j: int, frames: int, dev: torch.device):
-        key = (n, steps, r, j, frames, dev)
-        if self._ip is not None and self._ip["key"] == key:
-            return self._ip
-        f = self.cfg.num_h
-        prog = repaint_program(self.gamma, r, j, steps, frames)
-        st = dict(key=key, prog=prog,
-                  z=torch.zeros((n, 3 + f), device=dev), xh=torch.zeros((n, 3 + f), device=dev),
-                  nx=torch.zeros((n, 3), device=dev), nh=torch.zeros((n, f), device=dev),
-                  kx=torch.zeros((n, 3), device=dev), kh=torch.zeros((n, f), device=dev),
-                  step=torch.zeros((), dtype=torch.int32, device=dev), jstep=torch.zeros((), dtype=torch.int32, device=dev),
-                  coef=prog["rev"].to(dev), known=prog["known"].to(dev), jump=prog["jump"].to(dev),
-                  slot=prog["slot"].to(dev), dec=decode_coefficients(self.gamma).to(dev),
-                  xh0=torch.zeros((n, 3 + f), device=dev), fixed=torch.zeros(n, dtype=torch.uint8, device=dev),
-                  mf=torch.ones((n, 1), device=dev), topo=None,
-                  frames=torch.zeros((frames + 1, n, 3 + f), device=dev) if frames > 1 else None)
-        self._ip = st
-        self._ip_graphs = None
-        self._ip_graph_key = None
-        return st
-
     @torch.inference_mode()
     def inpaint(self, molecule: dict, node_mask_fixed: torch.Tensor, num_resamplings: int = 1, jump_length: int = 1,
                 return_frames: int = 1, num_timesteps: Optional[int] = None, context: Optional[torch.Tensor] = None,
@@ -384,32 +380,16 @@ class GCDMSampler:
         order: z_T, then per denoise op the known part and the unknown part, per jump one pair, the final decode.
         Returns out [N, 3+A(+1)], or [F, N, 3+A(+1)] for return_frames = F > 1 (frame 0 = the molecules).
         """
-        cfg = self.cfg
-        steps = cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
+        steps = self.cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
         r, j, nfr = int(num_resamplings), int(jump_length), int(return_frames)
         check_repaint(r, j, steps, nfr)
-        num_nodes, batch_index, parts, fixed, context = self._inpaint_inputs(cfg, molecule, node_mask_fixed, context)
+        num_nodes, batch_index, parts, fixed, context = self._inpaint_inputs(self.cfg, molecule, node_mask_fixed, context)
         dev = self._device()
-        if dev.type != "cuda":
-            raise _lib.BdiffError("GCDMSampler needs the denoiser on a CUDA device (no CPU fallback)")
         b = int(num_nodes.shape[0])
         n = int(batch_index.shape[0])
-        f = cfg.num_h
         batch_index = batch_index.to(dev)
         mask = torch.ones(n, dtype=torch.bool, device=dev)          # inpaint has no padding mask (:1638)
-        ctx, ctx_ptr = None, None
-        if cfg.num_context:
-            ctx = context.to(dev, torch.float32)[batch_index].contiguous()     # (:1614-1615)
-            ctx_ptr = C.c_void_p(ctx.data_ptr())
-        self.net.sync_weights()
-        st = self._inpaint_statics(n, steps, r, j, nfr, dev)
-        if st["topo"] is not None and torch.equal(st["topo"][0], batch_index):
-            batch_index, mask = st["topo"]
-        self.net.plan(batch_index, mask, b)
-        st["topo"] = (batch_index, mask)
-        prog = st["prog"]
-        lib = _lib.load()
-        h = self.net._handle
+        st, batch_index, mask = self._prepare(batch_index, mask, b, context, steps, (r, j), nfr)   # context: (:1614-1615)
 
         # xh0 with x centred on the fixed atoms of its molecule (:1617-1633); a molecule without fixed atoms is not moved.
         # A one-off step on the host: sequential float32 sums like the reference, and run-to-run reproducible (the
@@ -422,90 +402,4 @@ class GCDMSampler:
         xh0[:, :3] -= (tot / cnt.clamp(min=1.0).unsqueeze(-1))[bi_h]
         st["xh0"].copy_(xh0)
         st["fixed"].copy_(fixed.cpu().to(torch.uint8))
-
-        def draw(buf_x, buf_h):
-            if noise is None:
-                torch.randn((n, 3), device=dev, out=buf_x)
-                torch.randn((n, f), device=dev, out=buf_h)
-            else:
-                buf_x.copy_(noise((n, 3)))
-                buf_h.copy_(noise((n, f)))
-
-        def ptr(t):
-            return C.c_void_p(t.data_ptr())
-
-        def denoise_op():
-            draw(st["kx"], st["kh"])                                  # z_known's noise (:1661-1667)
-            draw(st["nx"], st["nh"])                                  # z_unknown = p(z_s | z_t) (:1670-1679)
-            self._reverse_step(st, ctx_ptr)
-            _lib.check(h, lib.bdiff_repaint_combine(h, self.net._stream(), ptr(st["z"]), ptr(st["xh0"]), ptr(st["fixed"]),
-                                                    ptr(st["kx"]), ptr(st["kh"]), ptr(st["known"]), ptr(st["step"])),
-                       "bdiff_repaint_combine")
-            if nfr > 1:
-                self._write_frame(st["frames"], st["slot"], st["step"], st["z"], st["mf"])
-            st["step"].add_(1)
-
-        def jump_back():
-            draw(st["nx"], st["nh"])
-            _lib.check(h, lib.bdiff_renoise(h, self.net._stream(), ptr(st["z"]), ptr(st["nx"]), ptr(st["nh"]), ptr(st["jump"]),
-                                            ptr(st["jstep"])), "bdiff_renoise")
-            st["jstep"].add_(1)
-
-        # z_T ~ N(0, I) on the zero-CoG subspace (:1635-1640)
-        draw(st["nx"], st["nh"])
-        _lib.check(h, lib.bdiff_center_noise(h, self.net._stream(), ptr(st["nx"]), ptr(st["nh"]), ptr(st["z"])), "bdiff_center_noise")
-        st["step"].zero_()
-        st["jstep"].zero_()
-        if nfr > 1:
-            st["frames"].zero_()
-
-        if self.use_cuda_graph and noise is None:
-            gkey = (st["key"], self.net._plan_key, self.net._plan_epoch, self.net._weights_key,
-                    ctx.data_ptr() if ctx is not None else 0)
-            if self._ip_graphs is None or self._ip_graph_key != gkey:
-                torch.cuda.current_stream().synchronize()
-                g_op = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g_op):
-                    denoise_op()
-                g_jump = None
-                if prog["num_jumps"]:
-                    g_jump = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g_jump):
-                        jump_back()
-                self._ip_graphs, self._ip_graph_key = (g_op, g_jump), gkey
-                self._ip_ctx_keep = ctx
-            g_op, g_jump = self._ip_graphs
-            for jump in prog["jump_after"]:
-                g_op.replay()
-                if jump:
-                    g_jump.replay()
-        else:
-            for jump in prog["jump_after"]:
-                denoise_op()
-                if jump:
-                    jump_back()
-
-        ops = len(prog["jump_after"])
-        per_forward = self.net.kernels_per_forward
-        self.kernel_launches += 1 + ops * (per_forward + 2) + prog["num_jumps"] + (per_forward + 1)
-        # p(x, h | z_0) (:1753-1762), then the CoG fix when no frames are returned (:1768-1778)
-        draw(st["nx"], st["nh"])
-        _lib.check(h, lib.bdiff_decode_z0(h, self.net._stream(), ptr(st["z"]), ctx_ptr, ptr(st["nx"]), ptr(st["nh"]), ptr(st["dec"]),
-                                          ptr(st["xh"])), "bdiff_decode_z0")
-        out = self._finish(st["xh"], batch_index, mask, b, cog_fix=nfr == 1)
-        if nfr > 1:
-            out = torch.cat((out.unsqueeze(0), st["frames"][1:nfr]), dim=0)          # out[0] <- the molecules (:1780-1786)
-        return out
-
-    def sample_from_host(self, num_nodes_host: torch.Tensor, context_host: Optional[torch.Tensor] = None,
-                         num_timesteps: Optional[int] = None, out_host: Optional[torch.Tensor] = None):
-        """End-to-end entry used by bench.py: pinned host inputs -> device -> chain -> pinned host result."""
-        dev = self._device()
-        nn_dev = num_nodes_host.to(dev, non_blocking=True)
-        ctx_dev = context_host.to(dev, non_blocking=True) if context_host is not None else None
-        out, batch_index, mask = self.sample(nn_dev, ctx_dev, num_timesteps)
-        if out_host is None:
-            out_host = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
-        out_host.copy_(out, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return out_host
+        return self._chain(st, noise, batch_index, mask, b)

@@ -60,7 +60,7 @@ def test_inpaint_matches_reference_golden(name, mode):
     torch.manual_seed(fx["noise_seed"])
     out = sampler.inpaint(molecule_cuda(fx), fx["node_mask_fixed"].cuda(), fx["num_resamplings"], fx["jump_length"],
                           fx["return_frames"], fx["steps"], ctx, noise=lambda s: torch.randn(s).cuda())
-    z0 = sampler._ip["z"]
+    z0 = sampler._static["z"]
     assert rel(z0, fx["z_0"]) <= 1e-4, f"z_0 rel diff {rel(z0, fx['z_0']):.3e}"
     check_out(ocfg, out, fx["out"])
 
@@ -236,11 +236,11 @@ def test_inpaint_graph_replay_equals_eager():
     fixed = (torch.rand(n, generator=g) < 0.4).cuda()
     s_graph = bdiff.GCDMSampler(net)
     s_graph.inpaint(mol, fixed, 2, 2, num_timesteps=6)                     # capture
-    assert s_graph._ip_graphs[1] is not None
+    assert len(s_graph._graphs) == 2                                      # the denoise op and the jump back
     outs = []
     for s in (s_graph, bdiff.GCDMSampler(net, use_cuda_graph=False)):
         torch.manual_seed(11)
-        outs.append((s.inpaint(mol, fixed, 2, 2, num_timesteps=6), s._ip["z"].clone()))
+        outs.append((s.inpaint(mol, fixed, 2, 2, num_timesteps=6), s._static["z"].clone()))
     assert torch.isfinite(outs[0][0]).all()
     assert torch.equal(outs[0][1], outs[1][1]) and torch.equal(outs[0][0], outs[1][0])
 

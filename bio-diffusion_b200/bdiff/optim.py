@@ -3,6 +3,7 @@ EMA of the weights as three multi-tensor kernels (`bdiff_optimizer_step`, csrc/b
 reference does with `configure_gradient_clipping` (qm9_mol_gen_ddpm.py:1267-1304), `torch.optim.AdamW`
 (configs/model/*_mol_gen_ddpm.yaml:3-8) and the `EMA` callback (src/utils/__init__.py:71-160) every step.
 No host synchronisation in `step()`; the gradient-norm history lives on the device."""
+import contextlib
 import ctypes as C
 from typing import Iterable
 
@@ -12,6 +13,7 @@ import torch
 from . import _lib
 
 STATE_WORDS = 8 + 120
+STATE_DICT_VERSION = 1
 
 
 class OptHyper(C.Structure):
@@ -42,8 +44,8 @@ class GCDMTrainTail:
             raise ValueError("queue_len must be in [1, 120]")
         self.lib = _lib.load()
         self.device = dev
-        self.hyper = OptHyper(lr, betas[0], betas[1], eps, weight_decay, ema_decay, int(bool(amsgrad)),
-                              int(bool(clip_gradients)), int(queue_len))
+        self._set_hyper(dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay, amsgrad=bool(amsgrad),
+                             ema_decay=ema_decay, clip=bool(clip_gradients), queue_len=int(queue_len)))
         z = lambda p: torch.zeros_like(p)
         # all gradients in ONE flat buffer (each tensor at a multiple of 64 floats): zero_grad is one memset and the DDP
         # exchange one all-reduce of the buffer itself, no packing
@@ -66,6 +68,14 @@ class GCDMTrainTail:
         st[8:9] = np.array([3000.0], dtype=np.float32).view(np.int32)
         self.state = torch.from_numpy(st).to(dev)
         self.kernel_launches = 0
+        self._ema_swapped = False
+
+    def _set_hyper(self, hp):
+        # the Python floats are kept as given so that a checkpoint written from them reproduces its source bit for bit;
+        # the kernels read the float32 copy in OptHyper
+        self.hyperparameters = dict(hp)
+        self.hyper = OptHyper(hp["lr"], hp["betas"][0], hp["betas"][1], hp["eps"], hp["weight_decay"], hp["ema_decay"],
+                              int(hp["amsgrad"]), int(hp["clip"]), hp["queue_len"])
 
     def _build_table(self):
         """Device-side pointer table; rebuilt if a parameter's storage moved (GCPNetDynamicsB200.flatten_parameters)."""
@@ -95,6 +105,8 @@ class GCDMTrainTail:
         return allreduce_mean_flat_(self.grad_flat, group)
 
     def step(self):
+        if self._ema_swapped:
+            raise _lib.BdiffError("the EMA weights are swapped in; swap them back (swap_ema()) before step()")
         for p, g in zip(self.params, self.grads):
             if p.grad is None or p.grad.data_ptr() != g.data_ptr():
                 raise _lib.BdiffError("p.grad was replaced; keep the buffers GCDMTrainTail installed (use opt.zero_grad())")
@@ -114,6 +126,89 @@ class GCDMTrainTail:
 
     def ema_parameters(self):
         return self.ema
+
+    def swap_ema(self):
+        """Exchange the parameters and the EMA weights in place (the reference's `replace_model_weights` /
+        `restore_original_weights`, src/utils/__init__.py:206-235); calling it twice restores both bit for bit.  The
+        parameters' version counters move, so GCPNetDynamicsB200.sync_weights repacks.  step() refuses to run while the
+        EMA weights are swapped in."""
+        with torch.no_grad():
+            for p, e in zip(self.params, self.ema):
+                tmp = p.detach().clone()
+                p.detach().copy_(e)
+                e.copy_(tmp)
+        torch.autograd.graph.increment_version(self.params)
+        self._ema_swapped = not self._ema_swapped
+
+    @contextlib.contextmanager
+    def ema_applied(self):
+        """`with opt.ema_applied(): evaluate(net)` — the parameters hold the EMA weights inside the block only."""
+        self.swap_ema()
+        try:
+            yield self
+        finally:
+            self.swap_ema()
+
+    def state_dict(self) -> dict:
+        """Everything `step()` reads besides the parameters and gradients, as detached clones on the parameters' device:
+        hyperparameters, per-tensor shapes, the AdamW moments (and amsgrad maxima), the EMA weights and a copy of the
+        control words (`state`: step count, history length, ring position, last norm / limit / coefficient / clipped
+        flag and the gradient-norm history, laid out as `bdiff_optimizer_step` documents in include/bdiff.h)."""
+        if self._ema_swapped:
+            raise _lib.BdiffError("the EMA weights are swapped in; swap them back (swap_ema()) before state_dict()")
+        clone = lambda ts: [t.detach().clone() for t in ts]
+        return {"version": STATE_DICT_VERSION, "hyperparameters": dict(self.hyperparameters),
+                "shapes": [tuple(p.shape) for p in self.params], "exp_avg": clone(self.exp_avg),
+                "exp_avg_sq": clone(self.exp_avg_sq),
+                "max_exp_avg_sq": clone(self.max_exp_avg_sq) if self.max_exp_avg_sq is not None else None,
+                "ema": clone(self.ema), "state": self.state.detach().clone()}
+
+    def _check_state_dict(self, sd: dict) -> None:
+        """Raise ValueError naming the first difference between `sd` and this tail's structure; changes nothing."""
+        if sd.get("version") != STATE_DICT_VERSION:
+            raise ValueError(f"state_dict version {sd.get('version')!r}, expected {STATE_DICT_VERSION}")
+        hp = sd["hyperparameters"]
+        for k in ("amsgrad", "queue_len"):
+            if hp[k] != self.hyperparameters[k]:
+                raise ValueError(f"{k}: state_dict has {hp[k]!r}, this GCDMTrainTail has {self.hyperparameters[k]!r}")
+        if len(sd["shapes"]) != len(self.params):
+            raise ValueError(f"state_dict holds {len(sd['shapes'])} tensors, this GCDMTrainTail {len(self.params)}")
+        for i, (s, p) in enumerate(zip(sd["shapes"], self.params)):
+            if tuple(s) != tuple(p.shape):
+                raise ValueError(f"tensor {i}: state_dict shape {tuple(s)}, parameter shape {tuple(p.shape)}")
+        keys = ["exp_avg", "exp_avg_sq", "ema"] + (["max_exp_avg_sq"] if hp["amsgrad"] else [])
+        for k in keys:
+            ts = sd[k]
+            if ts is None or len(ts) != len(self.params):
+                raise ValueError(f"{k}: expected {len(self.params)} tensors")
+            for i, (t, p) in enumerate(zip(ts, self.params)):
+                if tuple(t.shape) != tuple(p.shape) or t.dtype != torch.float32:
+                    raise ValueError(f"{k}[{i}]: {tuple(t.shape)} {t.dtype}, expected {tuple(p.shape)} torch.float32")
+        st = sd["state"]
+        if tuple(st.shape) != (STATE_WORDS,) or st.dtype != torch.int32:
+            raise ValueError(f"state: {tuple(st.shape)} {st.dtype}, expected ({STATE_WORDS},) torch.int32")
+        w = st.cpu()
+        step, n, pos, q = int(w[0]), int(w[1]), int(w[2]), hp["queue_len"]
+        if step < 0 or not 0 <= n <= q or not 0 <= pos < q:
+            raise ValueError(f"state: step {step}, history length {n}, ring position {pos} do not fit queue_len {q}")
+
+    def load_state_dict(self, sd: dict) -> None:
+        """Validate `sd` against this tail (tensor count, shapes, amsgrad, queue_len: ValueError on a mismatch, nothing
+        loaded), then copy it in place: the buffers, the device pointer table and the `p.grad` buffers stay the same
+        objects.  The saved hyperparameters replace the constructor's, as torch.optim does."""
+        if self._ema_swapped:
+            raise _lib.BdiffError("the EMA weights are swapped in; swap them back (swap_ema()) before load_state_dict()")
+        self._check_state_dict(sd)
+        with torch.no_grad():
+            for k in ("exp_avg", "exp_avg_sq", "max_exp_avg_sq", "ema"):
+                dst = getattr(self, k)
+                if dst is not None:
+                    for d, s in zip(dst, sd[k]):
+                        d.copy_(s)
+            self.state.copy_(sd["state"])
+        hp = dict(sd["hyperparameters"])
+        hp["betas"] = tuple(hp["betas"])
+        self._set_hyper(hp)
 
     def report(self):
         """Host copy of the control state (synchronises): step count, last gradient norm / limit / coefficient."""

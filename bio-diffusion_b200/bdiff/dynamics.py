@@ -173,6 +173,7 @@ class GCPNetDynamicsB200(nn.Module):
         n = bi.shape[0]
         b = int(num_mols) if num_mols is not None else int(bi[-1].item()) + 1
         e = C.c_int64(0)
+        self._plan_key = None        # a failed call may leave no plan (or not this one): never reuse the old key
         _lib.check(h, lib.bdiff_plan_topology(h, self._stream(), b, n, C.c_void_p(bi.data_ptr()),
                                               C.c_void_p(mk.data_ptr()), C.byref(e)), "bdiff_plan_topology")
         self._plan_key = key

@@ -12,6 +12,7 @@
 
 #include "../../include/bdiff.h"
 #include "bdiff_handle.h"
+#include "bdiff_plan.h"
 
 using namespace bdiff;
 
@@ -163,9 +164,9 @@ bool resolve(bdiff_handle* h, const std::string& name, std::vector<PackOp>& ops,
   return false;
 }
 
-cudaError_t ensure_work(bdiff_handle* h) {
+// Np / Ep: rows of the node / edge buffers
+cudaError_t ensure_work(bdiff_handle* h, size_t Np, size_t Ep) {
   const Dims& d = h->d;
-  const size_t Np = h->Npad, Ep = (size_t)h->Epad;
   size_t off = 0;
   auto take = [&](size_t n) { size_t o = off; off += (n + 63) / 64 * 64; return o; };
   const size_t o_xi = take(Np * 3), o_x = take(Np * 3), o_hin = take(Np * d.Hin), o_chin = take(Np * 6),
@@ -299,7 +300,7 @@ void bdiff_destroy(bdiff_handle* h) {
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
   if (h->side) cudaStreamDestroy(h->side);
-  h->plan_buf.release(); h->rc_buf.release(); h->layers_dev.release(); h->sched_buf.release(); h->items_buf.release(); h->work_buf.release(); h->eps_buf.release(); h->tu_buf.release(); h->tc_blob.release(); h->tc_node_blob.release(); h->stage_buf.release(); h->jobs_dev.release();
+  h->plan_buf.release(); h->rc_buf.release(); h->layers_dev.release(); h->sched_buf.release(); h->work_buf.release(); h->eps_buf.release(); h->tu_buf.release(); h->tc_blob.release(); h->tc_node_blob.release(); h->stage_buf.release(); h->jobs_dev.release();
   delete h;
 }
 
@@ -401,191 +402,66 @@ int32_t bdiff_weights_missing(const bdiff_handle* h) {
 int32_t bdiff_plan_topology(bdiff_handle* h, void* stream, int32_t num_mols, int64_t num_nodes,
                             const int64_t* batch_index, const uint8_t* mask, int64_t* num_edges_host) {
   if (!h) return BDIFF_EINVAL;
-  if (num_mols < 1 || num_nodes < 1 || !batch_index || !mask) return h->fail(BDIFF_EINVAL, "bad plan arguments");
-  if (num_nodes > (1ll << 30)) return h->fail(BDIFF_EINVAL, "too many nodes");
+  if (!batch_index || !mask) return h->fail(BDIFF_EINVAL, "bad plan arguments");
+  if (const char* why = plan_args_error(num_mols, num_nodes)) return h->fail(BDIFF_EINVAL, "%s", why);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int N = (int)num_nodes, B = num_mols;
+  const int N = (int)num_nodes;
   std::vector<int64_t> bi(N);
   std::vector<uint8_t> mk(N);
   cudaError_t e = cudaMemcpyAsync(bi.data(), batch_index, N * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(mk.data(), mask, N, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "plan D2H: %s", cudaGetErrorString(e));
-  std::vector<int> mol_off(B + 1, 0), act_off(B + 1, 0), act_idx, node_mol(N);
-  std::vector<long long> edge_off(B + 1, 0);
-  act_idx.reserve(N);
-  int64_t prev = 0;
-  for (int i = 0; i < N; ++i) {
-    const int64_t m = bi[i];
-    if (m < 0 || m >= B) return h->fail(BDIFF_EINVAL, "batch_index[%d]=%lld outside [0,%d)", i, (long long)m, B);
-    if (m < prev) return h->fail(BDIFF_EINVAL, "batch_index must be sorted (node %d)", i);
-    prev = m;
-    mol_off[m + 1]++;
-    node_mol[i] = (int)m;
-  }
-  for (int k = 0; k < B; ++k) mol_off[k + 1] += mol_off[k];
-  for (int k = 0; k < B; ++k) {
-    for (int i = mol_off[k]; i < mol_off[k + 1]; ++i)
-      if (mk[i]) act_idx.push_back(i);
-    act_off[k + 1] = (int)act_idx.size();
-    const long long na = act_off[k + 1] - act_off[k];
-    edge_off[k + 1] = edge_off[k] + na * na;
-  }
-  const long long E = edge_off[B];
-  if (E >= (1ll << 36)) return h->fail(BDIFF_EINVAL, "too many edges");
-  const size_t M = act_idx.size();
-  // device layout: [mol_off | act_off | act_idx | node_mol | edge_off(int64) | mask]
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) / 256 * 256; return o; };
-  const long long ntile128 = (E + 127) / 128;
-  std::vector<int> tile_mol((size_t)ntile128 + 1, 0);
-  {
-    int k = 0;
-    for (long long t = 0; t < ntile128; ++t) {
-      const long long g = t * 128;
-      while (k < B && edge_off[k + 1] <= g) ++k;
-      tile_mol[(size_t)t] = k;
-    }
-  }
-  // dependency tables of the layer megakernel: edge tile -> 32-node tiles of its molecules, node tile -> edge tiles
-  const int ntile32 = (N + 31) / 32;
-  std::vector<int> edge_dep((size_t)2 * (ntile128 + 1), 0), node_dep((size_t)2 * (ntile32 + 1), 0);
-  for (long long t = 0; t < ntile128; ++t) {
-    const long long g1 = std::min<long long>(E, t * 128 + 128) - 1;
-    int k0 = tile_mol[(size_t)t], k1 = k0;
-    while (k1 < B - 1 && edge_off[k1 + 1] <= g1) ++k1;
-    edge_dep[2 * t] = mol_off[k0] / 32;
-    edge_dep[2 * t + 1] = (mol_off[k1 + 1] - 1) / 32;
-  }
-  for (int u = 0; u < ntile32; ++u) {
-    const int n1 = std::min(N, u * 32 + 32) - 1;
-    const int k0 = node_mol[u * 32], k1 = node_mol[n1];
-    const long long e0 = edge_off[k0], e1 = edge_off[k1 + 1] - 1;
-    node_dep[2 * u] = e1 >= e0 ? (int)(e0 / 128) : 0;
-    node_dep[2 * u + 1] = e1 >= e0 ? (int)(e1 / 128) : -1;
-  }
-  // per node: edge tiles strictly inside its row (their sums go through Work::mid, see edge_tile_epilogue.inc)
-  const int Npad128 = round_up(N, 128) + 128;          // node buffers carry one spare 128-row block (ghost node tile of an odd pair)
-  std::vector<int> node_mid((size_t)2 * Npad128, 0);
-  for (int k = 0; k < B; ++k) {
-    const long long na = act_off[k + 1] - act_off[k];
-    for (long long a = 0; a < na; ++a) {
-      const long long g0 = edge_off[k] + a * na, g1 = g0 + na - 1;
-      const long long t0 = g0 / 128, t1 = g1 / 128;
-      if (t1 - t0 >= 2) {
-        const int i = act_idx[act_off[k] + a];
-        node_mid[2 * (size_t)i] = (int)(t0 + 1);
-        node_mid[2 * (size_t)i + 1] = (int)(t1 - t0 - 1);
-      }
-    }
-  }
-  const size_t o_mo = take((B + 1) * 4), o_ao = take((B + 1) * 4), o_ai = take((M + 1) * 4), o_nm = take(N * 4),
-               o_eo = take((B + 1) * 8), o_tm = take((ntile128 + 1) * 4), o_mk = take(N),
-               o_ed = take((ntile128 + 1) * 8), o_nd = take((ntile32 + 1) * 8), o_mid = take((size_t)Npad128 * 8);
-  std::vector<unsigned char> stage(off, 0);
-  memcpy(stage.data() + o_mo, mol_off.data(), (B + 1) * 4);
-  memcpy(stage.data() + o_ao, act_off.data(), (B + 1) * 4);
-  if (M) memcpy(stage.data() + o_ai, act_idx.data(), M * 4);
-  memcpy(stage.data() + o_nm, node_mol.data(), N * 4);
-  memcpy(stage.data() + o_eo, edge_off.data(), (B + 1) * 8);
-  memcpy(stage.data() + o_tm, tile_mol.data(), (size_t)(ntile128 + 1) * 4);
-  memcpy(stage.data() + o_mk, mk.data(), N);
-  memcpy(stage.data() + o_ed, edge_dep.data(), edge_dep.size() * 4);
-  memcpy(stage.data() + o_nd, node_dep.data(), node_dep.size() * 4);
-  memcpy(stage.data() + o_mid, node_mid.data(), node_mid.size() * 4);
-  e = h->plan_buf.ensure(off);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h->plan_buf.p, stage.data(), off, cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "plan H2D: %s", cudaGetErrorString(e));
+  HostPlan hp;
+  const std::string why = plan_host(num_mols, num_nodes, bi.data(), mk.data(), h->d.L, h->num_sms, hp);
+  if (!why.empty()) return h->fail(BDIFF_EINVAL, "%s", why.c_str());
+
+  // From here on the buffers of the previous plan may be freed: a failure leaves no plan.
+  auto lose = [&](int code, const char* what, cudaError_t err) {
+    h->have_plan = false;
+    h->plan_epoch++;
+    return h->fail(code, "%s: %s", what, cudaGetErrorString(err));
+  };
+  const long long nrc = (long long)hp.TE * 128;
+  const size_t nsched = 1 + (size_t)hp.nitems;       // queue head + one completion flag per item
+  e = h->plan_buf.ensure(hp.at.bytes);
+  if (e == cudaSuccess) e = h->rc_buf.ensure((size_t)std::max(nrc, 1ll) * sizeof(int4));
+  if (e == cudaSuccess) e = h->sched_buf.ensure((nsched + 1) * sizeof(int));
+  if (e != cudaSuccess) return lose(BDIFF_ENOMEM, "plan buffers", e);
+  e = cudaMemcpyAsync(h->plan_buf.p, hp.block.data(), hp.at.bytes, cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) return lose(BDIFF_ECUDA, "plan H2D", e);
   unsigned char* base = static_cast<unsigned char*>(h->plan_buf.p);
-  Plan& p = h->plan;
-  p.B = B; p.N = N; p.E = E;
-  p.mol_off = reinterpret_cast<int*>(base + o_mo);
-  p.act_off = reinterpret_cast<int*>(base + o_ao);
-  p.act_idx = reinterpret_cast<int*>(base + o_ai);
-  p.node_mol = reinterpret_cast<int*>(base + o_nm);
-  p.edge_off = reinterpret_cast<long long*>(base + o_eo);
-  p.tile_mol = reinterpret_cast<int*>(base + o_tm);
-  p.mask = base + o_mk;
-  p.edge_rc = nullptr;
-  p.node_mid = reinterpret_cast<const int2*>(base + o_mid);
-  {
-    const long long nrc = (ntile128 + 1) * 128;       // + one ghost tile (row = -1): the second CTA of the last pair when the tile count is odd
-    e = h->rc_buf.ensure((size_t)(nrc > 0 ? nrc : 1) * sizeof(int4));
-    if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "plan edge records: %s", cudaGetErrorString(e));
-    launch_edge_rc(st, p, static_cast<int4*>(h->rc_buf.p), nrc);
-    p.edge_rc = static_cast<const int4*>(h->rc_buf.p);
-    e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "plan edge records: %s", cudaGetErrorString(e));
-  }
-  h->sched.edge_dep = reinterpret_cast<const int2*>(base + o_ed);
-  h->sched.node_dep = reinterpret_cast<const int2*>(base + o_nd);
-  h->sched.TE = (int)ntile128;
-  h->sched.TN = ntile32;
-  {
-    // Claim order of the layer megakernel, in PAIR items: item j holds tiles (2j, 2j+1) of one kind and layer, claimed one
-    // tile at a time (the second tile of the last pair is skipped when the count is odd).  Virtual time of edge pair (l, j) =
-    // l*PE + j; node pair (l, v) follows the last edge pair it reads by `lag` items (about one wave of num_sms tile claims:
-    // by then that pair has normally finished).
-    // Every dependency must precede its consumer in the list (deadlock freedom), which bounds the lag: edge pair (l+1, j)
-    // reads node pairs <= ndep(j), whose time is l*PE + edep(ndep) + lag  <  (l+1)*PE + j.
-    const int L = h->d.L, TE = (int)ntile128, TN = ntile32;
-    const int PE = (TE + 1) / 2, PN = (TN + 1) / 2;
-    // an item packs the layer into bits 24..29 (0..63, so up to the 64 layers bdiff_create accepts) and the pair into 0..23
-    if (L > 64 || ntile128 >= (1 << 24) || ntile32 >= (1 << 24)) return h->fail(BDIFF_EINVAL, "problem too large for the tile scheduler");
-    auto node_pair_last_edge_pair = [&](int v) {          // last edge pair a node pair depends on (-1: none)
-      int th = -1;
-      for (int u = 2 * v; u < std::min(TN, 2 * v + 2); ++u) th = std::max(th, node_dep[2 * u + 1]);
-      return th >= 0 ? th / 2 : -1;
-    };
-    auto edge_pair_last_node_pair = [&](int j) {
-      int uh = -1;
-      for (int t = 2 * j; t < std::min(TE, 2 * j + 2); ++t) uh = std::max(uh, edge_dep[2 * t + 1]);
-      return uh >= 0 ? uh / 2 : -1;
-    };
-    long long lag = std::max(1, h->num_sms / 2);
-    for (int j = 0; j < PE; ++j) {
-      const int vh = edge_pair_last_node_pair(j);
-      const int jh = (vh >= 0 && vh < PN) ? node_pair_last_edge_pair(vh) : -1;
-      if (jh >= 0) lag = std::min<long long>(lag, (long long)PE - 1 - (jh - j));
-    }
-    if (lag < 0) lag = 0;
-    std::vector<std::pair<long long, int>> order;
-    order.reserve((size_t)L * (PE + PN));
-    for (int l = 0; l < L; ++l) {
-      for (int j = 0; j < PE; ++j) order.emplace_back(2 * ((long long)l * PE + j), (0 << 30) | (l << 24) | j);
-      for (int v = 0; v < PN; ++v) {
-        const int jh = node_pair_last_edge_pair(v);     // -1: no edges at all -> right at the start of the layer
-        const long long tau = (long long)l * PE + (jh >= 0 ? jh + lag : 0);
-        order.emplace_back(2 * tau + 1, (1 << 30) | (l << 24) | v);
-      }
-    }
-    std::stable_sort(order.begin(), order.end(), [](const std::pair<long long, int>& a, const std::pair<long long, int>& b) { return a.first < b.first; });
-    std::vector<int> items(order.size());
-    for (size_t i = 0; i < order.size(); ++i) items[i] = order[i].second;
-    e = h->items_buf.ensure(std::max<size_t>(items.size(), 1) * sizeof(int));
-    if (e == cudaSuccess && !items.empty())
-      e = cudaMemcpy(h->items_buf.p, items.data(), items.size() * sizeof(int), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "scheduler work list: %s", cudaGetErrorString(e));
-    h->sched.nitems = (int)items.size();
-    h->sched.items = static_cast<const int*>(h->items_buf.p);
-  }
-  {
-    const size_t nsched = 2 + (size_t)h->d.L * (size_t)(ntile128 + ntile32);
-    e = h->sched_buf.ensure((nsched + 1) * sizeof(int));
-    if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "scheduler buffer: %s", cudaGetErrorString(e));
-    h->sched.sched = static_cast<int*>(h->sched_buf.p);
-    h->sched.err = h->sched.sched + nsched;
-    cudaMemset(h->sched.err, 0, sizeof(int));
-  }
-  h->Npad = round_up(N, 128) + 128;
-  h->Epad = (E + 127) / 128 * 128 + 128;
-  e = ensure_work(h);
-  if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "workspace: %s", cudaGetErrorString(e));
+  Plan p{};
+  p.B = hp.B; p.N = hp.N; p.E = hp.E;
+  p.mol_off = reinterpret_cast<const int*>(base + hp.at.mol_off);
+  p.act_off = reinterpret_cast<const int*>(base + hp.at.act_off);
+  p.act_idx = reinterpret_cast<const int*>(base + hp.at.act_idx);
+  p.node_mol = reinterpret_cast<const int*>(base + hp.at.node_mol);
+  p.edge_off = reinterpret_cast<const long long*>(base + hp.at.edge_off);
+  p.mask = base + hp.at.mask;
+  p.node_mid = reinterpret_cast<const int2*>(base + hp.at.node_mid);
+  launch_edge_rc(st, p, static_cast<int4*>(h->rc_buf.p), nrc);
+  p.edge_rc = static_cast<const int4*>(h->rc_buf.p);
+  e = cudaGetLastError();
+  LayerSched q = h->sched;
+  q.TE = hp.TE; q.TN = hp.TN; q.nitems = hp.nitems;
+  q.edge_dep = reinterpret_cast<const int2*>(base + hp.at.edge_dep);
+  q.node_dep = reinterpret_cast<const int2*>(base + hp.at.node_dep);
+  q.items = reinterpret_cast<const int*>(base + hp.at.items);
+  q.sched = static_cast<int*>(h->sched_buf.p);
+  q.err = q.sched + nsched;
+  if (e == cudaSuccess) e = cudaMemsetAsync(q.err, 0, sizeof(int), st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return lose(BDIFF_ECUDA, "plan upload", e);
+  // node buffers carry one spare 128-row block, edge buffers one spare 128-edge tile
+  e = ensure_work(h, round_up(hp.N, 128) + 128, (size_t)hp.TE * 128 + 128);
+  if (e != cudaSuccess) return lose(BDIFF_ENOMEM, "workspace", e);
+  h->plan = p;
+  h->sched = q;
+  h->Mact = hp.Mact;
   h->have_plan = true;
   h->plan_epoch++;
-  h->Mact = (int)M;
-  if (num_edges_host) *num_edges_host = E;
+  if (num_edges_host) *num_edges_host = hp.E;
   return BDIFF_OK;
 }
 
@@ -643,14 +519,13 @@ static int32_t forward_impl(bdiff_handle* h, cudaStream_t st, const float* xh, c
   if (fused) {
     // all L layers in one persistent kernel (bdiff_layers_tc.cu); its queue head + completion flags are zeroed first
     LayerSched& q = h->sched;
-    const size_t nsched = 2 + (size_t)d.L * (q.TE + q.TN);      // buffer sized in bdiff_plan_topology
     q.layers = static_cast<const LayerW*>(h->layers_dev.p);
     q.edge_blob = static_cast<const unsigned char*>(h->tc_blob.p);
     q.edge_blob_stride = h->tc_layer_bytes;
     q.node_blob = static_cast<const unsigned char*>(h->tc_node_blob.p);
     q.node_blob_stride = h->tc_node_layer_bytes;
     q.L = d.L;
-    cudaMemsetAsync(q.sched, 0, nsched * sizeof(int), st);
+    cudaMemsetAsync(q.sched, 0, (1 + (size_t)q.nitems) * sizeof(int), st);
     launch_layers_tc(st, p, d, h->embed, q, w, h->num_sms);
     mark();
     h->launches += 1;

@@ -24,7 +24,7 @@ constexpr int TM_COLS = 512;  // columns of the per-CTA accumulator scratch of t
 constexpr int kPStride = 328; // per-node projection record: 256 + hid0*3 (<=60) + 9 -> 328
 constexpr int kKC = 16;       // K rows of a weight chunk staged in shared memory (16 x 256 x 4 B = 16 KiB)
 
-// Topology plan (device arrays), built once per (batch_index, mask) by bdiff_plan_topology.
+// Topology plan (device arrays), built once per (batch_index, mask) by bdiff_plan_topology (host part: bdiff_plan.h).
 struct Plan {
   int B;                 // molecules
   int N;                 // nodes (masked ones included)
@@ -34,10 +34,9 @@ struct Plan {
   const int* act_idx;    // [M]   global ids of unmasked nodes, ascending
   const long long* edge_off;  // [B+1] prefix of nact^2
   const int* node_mol;   // [N]   molecule of each node
-  const int* tile_mol;   // [ceil(E/128)] molecule that contains edge 128*t (start of the linear molecule search)
   const unsigned char* mask;  // [N]
   const int4* edge_rc;   // [128*ceil(E/128)] per edge {row, col, b, nact} (row = -1 past E): b = position in the row segment
-  const int2* node_mid;  // [Npad] per node {first, count} of the 128-edge tiles that lie strictly inside its row (count > 0 only for n >= 130)
+  const int2* node_mid;  // [32*ceil(N/32)] per node {first, count} of the 128-edge tiles that lie strictly inside its row (count > 0 only for n >= 130)
 };
 
 // Per-layer packed weights (device pointers, K-major).
@@ -306,13 +305,6 @@ __device__ __forceinline__ int find_mol(const long long* __restrict__ edge_off, 
     else hi = mid;
   }
   return lo;
-}
-
-// Same result as find_mol, but a short forward scan from the tile's first molecule (1-3 dependent loads).
-__device__ __forceinline__ int find_mol_from(const long long* __restrict__ edge_off, int k0, long long g) {
-  int k = k0;
-  while (__ldg(edge_off + k + 1) <= g) ++k;
-  return k;
 }
 
 }  // namespace bdiff

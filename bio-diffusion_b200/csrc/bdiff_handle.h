@@ -67,16 +67,14 @@ struct bdiff_handle {
   std::map<std::string, std::pair<size_t, size_t>> param_layout;
   size_t param_floats = 0;
   TrainState* train = nullptr;
-  int plan_epoch = 0;    // bumped by every bdiff_plan_topology
+  int plan_epoch = 0;    // bumped by every bdiff_plan_topology that builds a plan or, failing, drops one
   int Mact = 0;          // unmasked nodes of the current plan
 
   // plan
   bool have_plan = false;
   Plan plan{};
-  DevBuf plan_buf, rc_buf, layers_dev, sched_buf, items_buf;
+  DevBuf plan_buf, rc_buf, layers_dev, sched_buf;
   LayerSched sched{};
-  int Npad = 0;
-  long long Epad = 0;
 
   // workspace
   DevBuf work_buf;

@@ -78,12 +78,13 @@ struct LayerSched {
   const unsigned char* node_blob;
   size_t node_blob_stride;
   int L, TE, TN;                   // layers, 128-edge tiles, 32-node tiles
-  int nitems;                      // items in the work list: L * (ceil(TE/2) + ceil(TN/2))
-  int* sched;                      // [0] queue head, [1] unused, [2 + l*(TE+TN) + i] completion flags; zeroed per forward
+  int nitems;                      // items in the work list: L * (TE + TN)
+  int* sched;                      // [0] queue head, [1 + l*(TE+TN) + i] completion flags; zeroed per forward
   int* err;                        // sticky error word (dependency wait timed out); cleared when the plan is built / reported
   const int2* edge_dep;            // [TE] inclusive range of 32-node tiles whose previous-layer output an edge tile reads
   const int2* node_dep;            // [TN] inclusive range of edge tiles whose messages a node tile reads
-  const int* items;                // [nitems] work list in claim order: type<<30 | layer<<24 | item j = tiles 2j, 2j+1, claimed one at a time (see bdiff_plan_topology)
+  const int* items;                // [nitems] work list in claim order, one tile per item: type<<30 | layer<<24 | tile
+                                   // (work_item and plan_host in bdiff_plan.h)
 };
 cudaError_t tc_layers_configure();
 void launch_layers_tc(cudaStream_t st, const Plan& p, const Dims& d, const EmbedW& ew, const LayerSched& q,

@@ -5,9 +5,9 @@
 // pipeline-ramp gaps.  Nothing in the network couples molecules inside a
 // layer (gcpnet.py:676-737, 893-930: messages, aggregation and node updates are per molecule), so layer l+1 of
 // a molecule only needs layer l of the same molecule.  This kernel therefore runs the edge-tile and node-tile bodies
-// (edge_tile_*.inc, node_r4_tile_*.inc) from a global work list of tile PAIRS, claimed one tile at a time
-//     for l in 0..L-1:  edge pairs (l, 0..PE-1) in order, node pair (l, v) inserted ~one wave of claims after the last
-//                       edge pair it depends on (so its wait is short and the CTA that claims it does not idle)
+// (edge_tile_*.inc, node_r4_tile_*.inc) from a global work list of tiles (built by plan_host, bdiff_plan.h)
+//     for l in 0..L-1:  edge tiles (l, 0..TE-1) in order, node tile (l, u) inserted ~one wave of claims after the last
+//                       edge tile it depends on (so its wait is short and the CTA that claims it does not idle)
 // claimed with one atomicAdd per tile, with per-tile completion flags as dependencies:
 //     edge (l, t)  waits for node (l-1, u) of every 32-node tile u that intersects the molecules of edge tile t;
 //     node (l, u)  waits for edge (l, t) of every edge tile t that intersects the molecules of node tile u.
@@ -70,8 +70,7 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int hid0 = d.hid0;
   const int per_layer = q.TE + q.TN;
-  const int total_items = q.nitems;                 // items of two tiles
-  int* const flags = q.sched + 2;
+  int* const flags = q.sched + 1;
 
   if (tid == 0) {
     for (int i = 0; i < TC_NSLOT; ++i) { mbar_init(&B.full[i], 1); mbar_init(&B.empty[i], RING_CONSUMERS); }
@@ -92,13 +91,10 @@ __global__ void __launch_bounds__(LAYERS_THREADS, 1) k_layers_tc(Plan p, Dims d,
         const uint32_t slot = k & 1;
         mbar_wait_backoff(&B.item_empty[slot], ((k >> 1) & 1) ^ 1);
         int type = -1, layer = 0, tile = 0;
-        for (;;) {
-          const int qi = atomicAdd(q.sched, 1);
-          if (qi >= 2 * total_items) break;
-          const int it = __ldg(q.items + (qi >> 1));
-          type = (it >> 30) & 1; layer = (it >> 24) & 63; tile = 2 * (it & 0xffffff) + (qi & 1);
-          if (tile < (type == 0 ? q.TE : q.TN)) break;
-          type = -1;                                  // the missing second tile of an odd tile count: claim the next one
+        const int qi = atomicAdd(q.sched, 1);
+        if (qi < q.nitems) {
+          const int it = __ldg(q.items + qi);
+          type = (it >> 30) & 1; layer = (it >> 24) & 63; tile = it & 0xffffff;
         }
         B.item[slot][0] = type; B.item[slot][1] = layer; B.item[slot][2] = tile;
         mbar_arrive(&B.item_full[slot]);
@@ -281,7 +277,7 @@ cudaError_t tc_layers_configure() {
 // one CTA per SM at most (the accumulator scratch holds `num_sms` CTAs)
 void launch_layers_tc(cudaStream_t st, const Plan& p, const Dims& d, const EmbedW& ew, const LayerSched& q,
                       const Work& w, int num_sms) {
-  const int grid = 2 * q.nitems < num_sms ? 2 * q.nitems : num_sms;
+  const int grid = q.nitems < num_sms ? q.nitems : num_sms;
   if (d.Ed == 64) k_layers_tc<64, 16><<<grid, LAYERS_THREADS, LAYERS_SMEM_BYTES, st>>>(p, d, ew, q, w);
   else k_layers_tc<16, 8><<<grid, LAYERS_THREADS, LAYERS_SMEM_BYTES, st>>>(p, d, ew, q, w);
 }

@@ -4,7 +4,8 @@
 A molecule with `na` active atoms has na x na edges, row by row; edge tiles hold 128 edges in eight 16-row windows, node
 tiles 32 atoms.  `layout_paths` restates those tiling rules in plain Python (see test_gpu_tc_layouts.py for the paths).
 `_inputs` builds a case's seeded inputs: masked xh rows zero, coordinates centred per molecule, t and context per molecule,
-for the case's configuration or any other (test_gpu_configs.py).
+for the case's configuration or any other (test_gpu_configs.py).  `host_plan` restates the topology plan with numpy
+(test_plan_cpu.py, test_train_hostcheck.py).
 """
 from dataclasses import dataclass, field
 from typing import List, Tuple
@@ -88,9 +89,9 @@ LAYOUTS = [
     _sparse("qm9"),
     _sparse("geom"),
     Layout("node_tile_edges", "geom", [31, 2, 33, 70, 40, 17], [],
-           ("odd TN", "molecule straddles a node tile border", "molecule spans 3 node tiles"), schedule=True),
+           ("molecule straddles a node tile border", "molecule spans 3 node tiles"), schedule=True),
     Layout("tiny_1", "qm9", [1], [], ("E = 1",), schedule=True),
-    Layout("tiny_2", "qm9", [2], [], ("odd TE",), schedule=True),
+    Layout("tiny_2", "qm9", [2], [], schedule=True),
     Layout("all_masked", "qm9", [3, 4], list(range(7)), ("E = 0",), schedule=True),
     Layout("cond_masked", "qm9_cond", [9, 14, 20, 7], [2, 11, 12, 30, 40, 48], ("masked atom",)),
 ] + [_fuzz(c, s) for c in ("qm9", "geom") for s in range(3)]
@@ -144,9 +145,7 @@ def layout_paths(sizes, mask, config="qm9"):
                 if c == TMT // WIN - 1:
                     paths.add("row crosses 7 window borders")
         e += na * na
-    te, tn = (e + TMT - 1) // TMT, (o[-1] + R4M - 1) // R4M
-    paths.add("odd TE" if te % 2 else "even TE")
-    paths.add("odd TN" if tn % 2 else "even TN")
+    tn = (o[-1] + R4M - 1) // R4M
     if e == 0:
         paths.add("E = 0")
     if e == 1:
@@ -162,6 +161,51 @@ def layout_paths(sizes, mask, config="qm9"):
         if all(mask[o[k]:o[k + 1]].sum() == 0 for k in range(mol_of[lo], mol_of[hi - 1] + 1)):
             paths.add("empty node tile")
     return paths
+
+
+def host_plan(bi: torch.Tensor, mask: torch.Tensor):
+    """The arrays bdiff_plan_topology builds (plan_host in csrc/bdiff_plan.h), restated with numpy: the plan, the per-edge
+    records k_edge_rc computes on the device, and the layer megakernel's tables.  edge_dep[t] / node_dep[u] are the
+    inclusive ranges of 32-node tiles / 128-edge tiles holding the molecules of edge tile t / node tile u ((0, -1): none);
+    node_mid[i] = (first, count) of the edge tiles strictly inside node i's row, for the TN * 32 rows of the node tiles."""
+    bi = bi.numpy().astype(np.int64)
+    mk = mask.numpy().astype(np.uint8)
+    B, N = int(bi.max()) + 1, bi.shape[0]
+    mol_off = np.zeros(B + 1, np.int32)
+    np.add.at(mol_off, bi + 1, 1)
+    mol_off = np.cumsum(mol_off).astype(np.int32)
+    act_idx = np.nonzero(mk)[0].astype(np.int32)
+    act_off = np.zeros(B + 1, np.int32)
+    np.add.at(act_off, bi[act_idx] + 1, 1)
+    act_off = np.cumsum(act_off).astype(np.int32)
+    na = np.diff(act_off).astype(np.int64)
+    edge_off = np.concatenate([[0], np.cumsum(na * na)]).astype(np.int64)
+    E = int(edge_off[-1])
+    rc = [np.zeros((0, 4), np.int32)]
+    for k in range(B):
+        act = act_idx[act_off[k]:act_off[k + 1]]
+        n = len(act)
+        rc.append(np.stack([np.repeat(act, n), np.tile(act, n), np.tile(np.arange(n), n), np.full(n * n, n)], 1))
+    rc = np.concatenate(rc).astype(np.int32)
+    te, tn = (E + TMT - 1) // TMT, (N + R4M - 1) // R4M
+    mol_of_edge = lambda g: np.searchsorted(edge_off[1:], g, side="right")   # molecule holding edge g (g < E)
+    g0 = np.arange(te, dtype=np.int64) * TMT
+    k0, k1 = mol_of_edge(g0), mol_of_edge(np.minimum(E, g0 + TMT) - 1)
+    edge_dep = np.stack([mol_off[k0] // R4M, (mol_off[k1 + 1] - 1) // R4M], 1).astype(np.int32).reshape(te, 2)
+    node_dep = np.zeros((tn, 2), np.int32)
+    for u in range(tn):
+        e0, e1 = edge_off[bi[u * R4M]], edge_off[bi[min(N, u * R4M + R4M) - 1] + 1] - 1
+        node_dep[u] = (e0 // TMT, e1 // TMT) if e1 >= e0 else (0, -1)
+    node_mid = np.zeros((tn * R4M, 2), np.int32)
+    for k in range(B):
+        n = int(na[k])
+        for a in range(n):
+            t0, t1 = (edge_off[k] + a * n) // TMT, (edge_off[k] + a * n + n - 1) // TMT
+            if t1 - t0 >= 2:
+                node_mid[act_idx[act_off[k] + a]] = (t0 + 1, t1 - t0 - 1)
+    return dict(B=B, N=N, E=E, Mact=int(act_idx.shape[0]), TE=te, TN=tn, mol_off=mol_off, act_off=act_off,
+                act_idx=act_idx, edge_off=edge_off, node_mol=bi.astype(np.int32), mask=mk, edge_rc=rc,
+                edge_dep=edge_dep, node_dep=node_dep, node_mid=node_mid)
 
 
 def _inputs(c: Layout, ocfg: O.OracleConfig = None):

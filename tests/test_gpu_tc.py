@@ -80,6 +80,25 @@ def test_tensor_forward_matches_reference(name):
     assert max_abs <= FWD_TOL * scale
 
 
+def test_rejected_plan_leaves_the_previous_batch_intact():
+    """A batch the planner rejects (unsorted batch_index) changes no plan state: the next forward on the batch planned
+    before is bit-identical to the one before the rejection."""
+    import bdiff
+    net, ocfg, _ = make_net("qm9", 7, "tensor")
+    g = torch.Generator().manual_seed(3)
+    bi = torch.repeat_interleave(torch.arange(4), torch.tensor([5, 9, 3, 19])).cuda()
+    n = bi.shape[0]
+    mask = torch.ones(n, dtype=torch.bool, device="cuda")
+    xh = torch.randn((n, 3 + ocfg.num_h), generator=g).cuda()
+    t = torch.full((n, 1), 0.5, device="cuda")
+    first = net.denoise(bi, mask, xh, t)
+    unsorted = bi.clone()
+    unsorted[4], unsorted[5] = 1, 0
+    with pytest.raises(bdiff.BdiffError, match="batch_index must be sorted"):
+        net.denoise(unsorted, mask, xh, t)
+    assert torch.equal(net.denoise(bi, mask, xh, t), first)
+
+
 @pytest.mark.parametrize("b", [128, 300])
 def test_tensor_and_parity_modes_agree_full_size(b):
     """QM9 B=128 (BASELINE config) and B=300 (more 32-node tiles than SMs): tensor mode vs parity mode on the same input,

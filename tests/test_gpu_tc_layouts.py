@@ -5,7 +5,7 @@ A molecule with `na` active atoms has na x na edges, row by row; edge tiles hold
 tiles 32 atoms.  The segmented sum of edge_tile_epilogue.inc takes one of several paths for a source atom's row: it lies in
 one window, crosses window borders (joined by `finish_crossing`), is cut by one tile border (two `atomicAdd` addends into
 `agg`), or a tile lies strictly inside it (the tile's sum goes to `Work::mid`, the node tile adds those in ascending order).
-The schedule adds ghost tiles for odd tile counts, node tiles without edges and dependency ranges spanning molecules.
+The schedule adds node tiles without edges and dependency ranges spanning molecules.
 
 LAYOUTS names batches that reach each of these paths.  `layout_paths` restates the tiling rules in plain Python (both
 live in layout_catalogue.py, shared with the training-step tests of test_gpu_train_layouts.py); the CPU test checks that
@@ -31,7 +31,7 @@ WEIGHT_SEED = {"qm9": 7, "qm9_cond": 5, "geom": 3}
 PATH_CLASSES = {
     "row inside one window", "row crosses 1 window border", "row crosses 2+ window borders",
     "row crosses 7 window borders", "whole-tile row", "row cut once", "row cut 1 + 127", "1 mid tile", "2 mid tiles",
-    "edge tile spans molecules", "odd TE", "even TE", "odd TN", "even TN", "E = 0", "E = 1", "empty molecule",
+    "edge tile spans molecules", "E = 0", "E = 1", "empty molecule",
     "empty node tile", "node tile without active atoms", "masked atom", "masked atom in the GEOM build",
     "one active atom", "molecule straddles a node tile border", "molecule spans 3 node tiles",
 }
@@ -61,7 +61,7 @@ def test_layout_paths_model():
     assert "2 mid tiles" not in layout_paths([258], [True] * 258)    # a lone molecule needs n >= 259
     assert "2 mid tiles" in layout_paths([259], [True] * 259)
     p = layout_paths([3, 4], [False] * 7)
-    assert {"E = 0", "empty molecule", "empty node tile", "even TE"} <= p
+    assert {"E = 0", "empty molecule", "empty node tile"} <= p
 
 
 def test_oracle_empty_molecule_guard():

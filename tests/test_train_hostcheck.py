@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import gcpnet_oracle as O
+from layout_catalogue import host_plan
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "oracle", "hostcheck", "train_hostcheck.cpp")
@@ -24,31 +25,6 @@ def build_hostcheck():
     if not os.path.exists(OUT) or os.path.getmtime(OUT) < max(os.path.getmtime(SRC), os.path.getmtime(HDR)):
         subprocess.check_call(["g++", "-O2", "-fopenmp", "-std=c++17", "-shared", "-fPIC", "-o", OUT, SRC])
     return C.CDLL(OUT)
-
-
-def host_plan(bi: torch.Tensor, mask: torch.Tensor):
-    """The arrays bdiff_plan_topology builds (csrc/bdiff_api.cu), restated with numpy for the host harness."""
-    bi = bi.numpy().astype(np.int64)
-    mk = mask.numpy().astype(np.uint8)
-    B, N = int(bi.max()) + 1, bi.shape[0]
-    mol_off = np.zeros(B + 1, np.int32)
-    np.add.at(mol_off, bi + 1, 1)
-    mol_off = np.cumsum(mol_off).astype(np.int32)
-    act_idx = np.nonzero(mk)[0].astype(np.int32)
-    act_off = np.zeros(B + 1, np.int32)
-    np.add.at(act_off, bi[act_idx] + 1, 1)
-    act_off = np.cumsum(act_off).astype(np.int32)
-    na = np.diff(act_off).astype(np.int64)
-    edge_off = np.concatenate([[0], np.cumsum(na * na)]).astype(np.int64)
-    rc = []
-    for k in range(B):
-        act = act_idx[act_off[k]:act_off[k + 1]]
-        for r in act:
-            for b, c in enumerate(act):
-                rc.append((r, c, b, len(act)))
-    rc = np.array(rc, np.int32).reshape(-1, 4)
-    return dict(B=B, N=N, E=int(edge_off[-1]), Mact=int(act_idx.shape[0]), mol_off=mol_off, act_off=act_off,
-                act_idx=act_idx, edge_off=edge_off, node_mol=bi.astype(np.int32), mask=mk, edge_rc=rc)
 
 
 def run_hostcheck(lib, cfg, sd, bi, mask, xh, t, ctx, d_out):

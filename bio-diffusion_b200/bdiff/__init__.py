@@ -2,7 +2,8 @@
 
 Public surface (mirrors the reference's seam, SURVEY.md §8b):
     GCPNetDynamicsB200   drop-in for src.models.components.gcpnet.GCPNetDynamics
-    GCDMSampler          inner loop of EquivariantVariationalDiffusion.mol_gen_sample
+    GCDMSampler          inner loop of EquivariantVariationalDiffusion.mol_gen_sample (sample(seed=) runs it natively)
+    philox_noise         NoiseFn replaying the counter-based draws of the native chain (bdiff_sample)
     GCDMEvalNLL          evaluation-mode NLL terms of EquivariantVariationalDiffusion.forward (forward only)
     GCDMTrainLoss        training-mode L2 objective of the same function (value only, no backward)
     check_molecular_stability_batch   the reference's check_molecular_stability for a whole sampled batch in one kernel
@@ -15,6 +16,7 @@ Public surface (mirrors the reference's seam, SURVEY.md §8b):
 from .config import DenoiserConfig, parameter_shapes
 from .dynamics import GCPNetDynamicsB200
 from .sampler import GCDMSampler
+from .noise import philox_noise
 from .loss import GCDMEvalNLL, GCDMTrainLoss
 from .optim import GCDMTrainTail
 from .checkpoint import (training_state, load_training_state, from_reference_checkpoint, to_reference_checkpoint,
@@ -24,4 +26,4 @@ from .classifier import PropertyClassifier
 from .datasets import QM9_N_NODES, GEOM_N_NODES, sample_num_nodes
 from ._lib import BdiffError, load as load_library
 
-__all__ = ["DenoiserConfig", "parameter_shapes", "GCPNetDynamicsB200", "GCDMSampler", "GCDMEvalNLL", "GCDMTrainLoss", "GCDMTrainTail", "training_state", "load_training_state", "from_reference_checkpoint", "to_reference_checkpoint", "reference_to_training_state", "training_state_to_reference", "check_molecular_stability_batch", "PropertyClassifier", "QM9_N_NODES", "GEOM_N_NODES", "sample_num_nodes", "BdiffError", "load_library"]
+__all__ = ["DenoiserConfig", "parameter_shapes", "GCPNetDynamicsB200", "GCDMSampler", "philox_noise", "GCDMEvalNLL", "GCDMTrainLoss", "GCDMTrainTail", "training_state", "load_training_state", "from_reference_checkpoint", "to_reference_checkpoint", "reference_to_training_state", "training_state_to_reference", "check_molecular_stability_batch", "PropertyClassifier", "QM9_N_NODES", "GEOM_N_NODES", "sample_num_nodes", "BdiffError", "load_library"]

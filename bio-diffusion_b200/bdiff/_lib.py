@@ -30,6 +30,12 @@ class ClassifierConfig(C.Structure):
                 ("n_layers", C.c_int32), ("attention", C.c_int32), ("node_attr", C.c_int32)]
 
 
+class SampleConfig(C.Structure):
+    _fields_ = [("num_atom_types", C.c_int32), ("include_charges", C.c_int32), ("model_timesteps", C.c_int32),
+                ("reserved", C.c_int32), ("schedule_power", C.c_double), ("noise_precision", C.c_double),
+                ("norm_values", C.c_float * 3), ("norm_biases", C.c_float * 3)]
+
+
 # name -> (restype, argtypes): exactly the symbols include/bdiff.h declares
 PROTOTYPES = {
     "bdiff_abi_version": (C.c_int32, []),
@@ -56,6 +62,13 @@ PROTOTYPES = {
     "bdiff_repaint_combine": (C.c_int32, [C.c_void_p] * 9),
     "bdiff_renoise": (C.c_int32, [C.c_void_p] * 7),
     "bdiff_check": (C.c_int32, [C.c_void_p, C.c_void_p]),
+    "bdiff_schedule_tables": (C.c_int32, [C.POINTER(SampleConfig), C.c_int32, C.c_void_p, C.c_void_p]),
+    "bdiff_sample_setup": (C.c_int32, [C.c_void_p, C.POINTER(SampleConfig)]),
+    "bdiff_noise_fill": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_void_p]),
+    "bdiff_philox_fill": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_void_p]),
+    "bdiff_sample": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
+                                 C.c_uint64, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bdiff_sample_graph_builds": (C.c_int64, [C.c_void_p]),
     "bdiff_check_stability": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32, C.c_int32] + [C.c_void_p] * 3 + [C.c_float] * 3 +
                               [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bdiff_bond_orders": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32, C.c_int32] + [C.c_void_p] * 3 + [C.c_float] * 3 +

@@ -20,6 +20,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from .dynamics import GCPNetDynamicsB200
+from .noise import sample_config
 from .schedule import (chain_frame_slots, check_frames, check_repaint, decode_coefficients, gamma_table,
                        repaint_program, step_coefficient_table)
 
@@ -241,7 +242,7 @@ class GCDMSampler:
     def sample(self, num_nodes: torch.Tensor, context: Optional[torch.Tensor] = None,
                num_timesteps: Optional[int] = None, node_mask: Optional[torch.Tensor] = None,
                noise: Optional[NoiseFn] = None, return_z0: bool = False, z_init: Optional[torch.Tensor] = None,
-               record_moments: bool = False, return_frames: int = 1):
+               record_moments: bool = False, return_frames: int = 1, seed: Optional[int] = None):
         """mol_gen_sample (variational_diffusion.py:1280-1412).
 
         num_nodes int64[B]; context [B,C] or None; `noise(shape)` optionally injects the randn draws (tests).
@@ -250,8 +251,18 @@ class GCDMSampler:
         Returns (out [N, 3+A(+1)], batch_index [N], node_mask [N]) like the reference (+ z_0 when asked).  With
         return_frames = F > 1, out is [F, N, 3+A(+1)]: frame k is the unnormalised latent after the step that lands on
         s = k*T/F, frame 0 the decoded molecules (no CoG drift correction, as in the reference).
+
+        `seed` = s runs the whole chain in the library instead (bdiff_sample): the noise is drawn inside the step kernels
+        from Philox4x32-10 keyed by s, so nothing is drawn from torch's generator.  The result is bit-identical to
+        `sample(..., noise=philox_noise(s))` and is reproducible from the seed and the batch.  Not combinable with
+        `noise`, `node_mask`, `return_z0`, `record_moments` or `return_frames` > 1.
         """
         steps = self.cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
+        if seed is not None:
+            if noise is not None or node_mask is not None or return_z0 or record_moments or return_frames != 1:
+                raise ValueError("sample(seed=...) runs the native chain: noise, node_mask, return_z0, record_moments and "
+                                 "return_frames > 1 are not available there")
+            return self._sample_native(num_nodes, context, steps, int(seed), z_init)
         check_frames(steps, return_frames)
         dev = self._device()
         num_nodes = num_nodes.to(dev, non_blocking=True)
@@ -265,6 +276,49 @@ class GCDMSampler:
         out = self._chain(st, noise, batch_index, mask, b, z_init)
         self.last_moments = st["moments"].clone() if record_moments else None
         return (out, batch_index, mask, st["z"].clone()) if return_z0 else (out, batch_index, mask)
+
+    def _sample_native(self, num_nodes: torch.Tensor, context: Optional[torch.Tensor], steps: int, seed: int,
+                       z_init: Optional[torch.Tensor]):
+        """sample(seed=...): one bdiff_sample call on this sampler's coefficient tables."""
+        cfg = self.cfg
+        dev = self._device()
+        if dev.type != "cuda":
+            raise _lib.BdiffError("GCDMSampler needs the denoiser on a CUDA device (no CPU fallback)")
+        if steps < 1:
+            raise ValueError(f"num_timesteps must be >= 1, got {steps}")
+        counts = num_nodes.detach().reshape(-1).to("cpu", torch.int32).contiguous()
+        b, n = int(counts.shape[0]), int(counts.sum())
+        if cfg.num_context:
+            if context is None or tuple(context.shape) != (b, cfg.num_context):
+                raise ValueError(f"property-conditional configuration: `context` [{b}, {cfg.num_context}] is required")
+            context = context.to(dev, torch.float32).contiguous()
+        elif context is not None:
+            raise ValueError("`context` given to a configuration without conditioning")
+        zi = None
+        zshape = None
+        if z_init is not None:
+            zi = z_init.to(dev, torch.float32).contiguous()
+            zshape = (C.c_int64 * 2)(*zi.shape) if zi.dim() == 2 else (C.c_int64 * 2)(-1, -1)
+        self.net.sync_weights()
+        lib = _lib.load()
+        h = self.net._handle
+        sc = sample_config(cfg)
+        _lib.check(h, lib.bdiff_sample_setup(h, C.byref(sc)), "bdiff_sample_setup")
+        # the Python chain's own tables, so that both chains run the same coefficients bit for bit
+        tables = torch.cat((step_coefficient_table(self.gamma, steps).reshape(-1), decode_coefficients(self.gamma)))
+        tables = tables.to(torch.float32).contiguous()
+        out = torch.empty((n, 3 + cfg.num_h), dtype=torch.float32, device=dev)
+        bi = torch.empty(n, dtype=torch.int64, device=dev)
+        before = lib.bdiff_launch_count(h)
+        # the library plans this batch itself: the module's plan cache and the graphs captured on it are stale after it
+        self.net._plan_key = None
+        self.net._plan_epoch += 1
+        rc = lib.bdiff_sample(h, self.net._stream(), b, counts.numpy().ctypes.data_as(C.POINTER(C.c_int32)), _ptr(context),
+                              steps, seed & 0xFFFFFFFFFFFFFFFF, _ptr(zi), zshape, C.c_void_p(tables.data_ptr()),
+                              _ptr(out), _ptr(bi))
+        _lib.check(h, rc, "bdiff_sample")
+        self.kernel_launches += int(lib.bdiff_launch_count(h) - before)
+        return out, bi, torch.ones(n, dtype=torch.bool, device=dev)
 
     def nan_guard_count(self, reset: bool = False) -> int:
         """Denoiser forwards in which the NaN guard of gcpnet.py:1214-1216 fired since the workspace was (re)planned."""
@@ -295,18 +349,19 @@ class GCDMSampler:
     @torch.inference_mode()
     def optimize(self, samples, num_nodes: torch.Tensor, context: Optional[torch.Tensor] = None,
                  num_timesteps: Optional[int] = None, node_mask: Optional[torch.Tensor] = None,
-                 noise: Optional[NoiseFn] = None, return_frames: int = 1):
+                 noise: Optional[NoiseFn] = None, return_frames: int = 1, seed: Optional[int] = None):
         """mol_gen_optimize (variational_diffusion.py:1414-1546, norm_with_original_timesteps=False):
         run `num_timesteps` reverse steps starting from existing molecules.  `samples` = list of (x [n_k,3] CoG-free,
         one_hot [n_k,A]) per molecule as in the reference.  Only configurations without integer features
         (include_charges=False) — the reference stacks positions and categorical features only.  return_frames as in
-        `sample` (:1471-1498)."""
+        `sample` (:1471-1498); `seed` as in `sample` (the native chain from the molecules' latent)."""
         cfg = self.cfg
         if cfg.include_charges:
             raise NotImplementedError("mol_gen_optimize stacks [x | one-hot] only: needs include_charges=False")
         check_frames(cfg.num_timesteps if num_timesteps is None else int(num_timesteps), return_frames)
         z = self._optimize_latent(cfg, samples, num_nodes, self._device(), node_mask)
-        return self.sample(num_nodes, context, num_timesteps, node_mask, noise, z_init=z, return_frames=return_frames)
+        return self.sample(num_nodes, context, num_timesteps, node_mask, noise, z_init=z, return_frames=return_frames,
+                           seed=seed)
 
     @staticmethod
     def _optimize_latent(cfg, samples, num_nodes: torch.Tensor, dev: torch.device,

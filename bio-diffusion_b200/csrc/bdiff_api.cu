@@ -13,6 +13,7 @@
 #include "../../include/bdiff.h"
 #include "bdiff_handle.h"
 #include "bdiff_plan.h"
+#include "bdiff_schedule.h"
 
 using namespace bdiff;
 
@@ -300,6 +301,10 @@ void bdiff_destroy(bdiff_handle* h) {
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
   if (h->side) cudaStreamDestroy(h->side);
+  if (h->smp_graph) cudaGraphExecDestroy(h->smp_graph);
+  if (h->smp_ev) cudaEventDestroy(h->smp_ev);
+  if (h->smp_stream) cudaStreamDestroy(h->smp_stream);
+  h->smp_buf.release();
   h->plan_buf.release(); h->rc_buf.release(); h->layers_dev.release(); h->sched_buf.release(); h->work_buf.release(); h->eps_buf.release(); h->tu_buf.release(); h->tc_blob.release(); h->tc_node_blob.release(); h->stage_buf.release(); h->jobs_dev.release();
   delete h;
 }
@@ -341,6 +346,7 @@ int32_t bdiff_set_weight(bdiff_handle* h, void* stream, const char* name, const 
   e = cudaMemcpyAsync(static_cast<float*>(h->stage_buf.p) + off, data, count * sizeof(float), cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "stage '%s': %s", name, cudaGetErrorString(e));
   it->second = true;
+  h->weights_epoch++;
   h->pack_dirty = true;
   h->tc_dirty = true;
   return BDIFF_OK;
@@ -698,5 +704,186 @@ int32_t bdiff_nan_guard_count(bdiff_handle* h, void* stream, int64_t* count_host
 }
 
 int64_t bdiff_launch_count(const bdiff_handle* h) { return h ? h->launches : 0; }
+
+// ------------------------------------------------------------------------------------------ native chain
+int32_t bdiff_schedule_tables(const bdiff_sample_config* cfg, int32_t num_timesteps, float* coef_out, float* decode_out) {
+  if (!cfg || !coef_out || !decode_out || num_timesteps < 1) return BDIFF_EINVAL;
+  if (sample_config_error(*cfg)) return BDIFF_EINVAL;
+  schedule_tables(schedule_gamma(cfg->model_timesteps, cfg->schedule_power, cfg->noise_precision), num_timesteps,
+                  coef_out, decode_out);
+  return BDIFF_OK;
+}
+
+int32_t bdiff_sample_setup(bdiff_handle* h, const bdiff_sample_config* cfg) {
+  if (!h || !cfg) return h ? h->fail(BDIFF_EINVAL, "null argument") : BDIFF_EINVAL;
+  if (const char* why = sample_config_error(*cfg)) return h->fail(BDIFF_EINVAL, "%s", why);
+  if (cfg->num_atom_types + cfg->include_charges != h->d.F)
+    return h->fail(BDIFF_EINVAL, "num_atom_types + include_charges = %d, but the handle's num_h is %d",
+                   cfg->num_atom_types + cfg->include_charges, h->d.F);
+  h->scfg = *cfg;
+  h->have_sample_cfg = true;
+  return BDIFF_OK;
+}
+
+int32_t bdiff_noise_fill(void* stream, uint64_t seed, uint64_t draw_index, int64_t rows, int64_t cols, float* out) {
+  if (!out || rows < 0 || cols < 0) return BDIFF_EINVAL;
+  launch_noise_fill(static_cast<cudaStream_t>(stream), seed, draw_index, rows * cols, out);
+  return cudaGetLastError() == cudaSuccess ? BDIFF_OK : BDIFF_ECUDA;
+}
+
+int32_t bdiff_philox_fill(void* stream, uint64_t seed, uint64_t draw_index, int64_t blocks, uint32_t* out) {
+  if (!out || blocks < 0) return BDIFF_EINVAL;
+  launch_philox_fill(static_cast<cudaStream_t>(stream), seed, draw_index, blocks, out);
+  return cudaGetLastError() == cudaSuccess ? BDIFF_OK : BDIFF_ECUDA;
+}
+
+int64_t bdiff_sample_graph_builds(const bdiff_handle* h) { return h ? h->smp_graph_builds : 0; }
+
+int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host, const float* context,
+                     int32_t num_timesteps, uint64_t seed, const float* z_init, const int64_t* z_init_shape,
+                     const float* tables_host, float* xh, int64_t* batch_index) {
+  if (!h) return BDIFF_EINVAL;
+  if (!h->have_sample_cfg) return h->fail(BDIFF_ESTATE, "bdiff_sample_setup has not been called");
+  const std::string why = sample_args_error(h->d.F, h->d.C, h->scfg, num_mols, num_nodes_host, context, num_timesteps,
+                                            z_init, z_init_shape, xh);
+  if (!why.empty()) return h->fail(BDIFF_EINVAL, "bdiff_sample: %s", why.c_str());
+  if (bdiff_weights_missing(h) != 0) return h->fail(BDIFF_ESTATE, "%d parameters not set", bdiff_weights_missing(h));
+  const int B = num_mols, T = num_timesteps, F = h->d.F, C = h->d.C, ld = 3 + F;
+  std::vector<int32_t> counts(num_nodes_host, num_nodes_host + B);
+  long long N = 0;
+  for (int32_t c : counts) N += c;
+
+  // the legacy default stream cannot be captured: run on the handle's own stream, ordered after it
+  cudaStream_t run = static_cast<cudaStream_t>(stream);
+  cudaError_t e = cudaSuccess;
+  if (!run) {
+    if (!h->smp_stream) {
+      e = cudaStreamCreateWithFlags(&h->smp_stream, cudaStreamNonBlocking);
+      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->smp_ev, cudaEventDisableTiming);
+      if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
+    }
+    run = h->smp_stream;
+    e = cudaEventRecord(h->smp_ev, cudaStreamLegacy);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(run, h->smp_ev, 0);
+    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
+  }
+
+  // chain buffers: batch_index, mask, z, decoded xh, per-atom context, {step, done, seed, draw0}, CoG sums, decode row,
+  // and last the coefficient table, so that no buffer the captured step reads moves with the chain length
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) / 256 * 256; return o; };
+  const size_t o_bi = take(N * 8), o_mask = take(N), o_z = take(N * ld * 4), o_xhn = take(N * ld * 4),
+               o_ctx = take(N * C * 4), o_ctr = take(24), o_tot = take((size_t)B * 12), o_dec = take(16),
+               o_coef = take((size_t)T * 16);
+  e = h->smp_buf.ensure(at);
+  if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "sample buffers: %s", cudaGetErrorString(e));
+  unsigned char* base = static_cast<unsigned char*>(h->smp_buf.p);
+  int64_t* bi_dev = reinterpret_cast<int64_t*>(base + o_bi);
+  float* z = reinterpret_cast<float*>(base + o_z);
+  float* xhn = reinterpret_cast<float*>(base + o_xhn);
+  float* ctx = C ? reinterpret_cast<float*>(base + o_ctx) : nullptr;
+  float* coef = reinterpret_cast<float*>(base + o_coef);
+  float* dec = reinterpret_cast<float*>(base + o_dec);
+  int* ctr = reinterpret_cast<int*>(base + o_ctr);                                   // {step, done}
+  unsigned long long* seed_draw = reinterpret_cast<unsigned long long*>(base + o_ctr + 8);   // {seed, draw0}
+  float* tot = reinterpret_cast<float*>(base + o_tot);
+
+  // batch_index and mask are written on every call: they live in smp_buf, which ensure() above may just have replaced
+  // with a zeroed allocation (a longer chain grows it) even when the plan below is reused
+  std::vector<int64_t> bi((size_t)N);
+  for (int k = 0, i = 0; k < B; ++k)
+    for (int j = 0; j < counts[k]; ++j) bi[i++] = k;
+  e = cudaMemcpyAsync(bi_dev, bi.data(), N * 8, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemsetAsync(base + o_mask, 1, N, run);
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample batch: %s", cudaGetErrorString(e));
+  // topology: replanned only when the batch changed or another plan replaced ours
+  if (!h->have_plan || counts != h->smp_counts || h->plan_epoch != h->smp_plan_epoch) {
+    h->smp_counts.clear();
+    int32_t rc = bdiff_plan_topology(h, run, B, N, bi_dev, base + o_mask, nullptr);
+    if (rc != BDIFF_OK) return rc;
+    h->smp_counts = counts;
+    h->smp_plan_epoch = h->plan_epoch;
+  }
+
+  std::vector<float> tables((size_t)T * 4 + 4);
+  if (tables_host) {
+    std::copy(tables_host, tables_host + tables.size(), tables.begin());
+  } else {
+    schedule_tables(schedule_gamma(h->scfg.model_timesteps, h->scfg.schedule_power, h->scfg.noise_precision), T,
+                    tables.data(), tables.data() + (size_t)T * 4);
+  }
+  e = cudaMemcpyAsync(coef, tables.data(), (size_t)T * 16, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dec, tables.data() + (size_t)T * 4, 16, cudaMemcpyHostToDevice, run);
+  // z_T = draws 0, 1 (masked, x centred), or the caller's start; the reverse steps' draws follow
+  const unsigned long long draw0 = z_init ? 0 : 2, sd[2] = {seed, draw0};
+  if (e == cudaSuccess) e = cudaMemsetAsync(ctr, 0, 8, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(seed_draw, sd, 16, cudaMemcpyHostToDevice, run);
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample tables: %s", cudaGetErrorString(e));
+  tc_prepare(h, run);
+  const Plan& p = h->plan;
+  if (C) {
+    launch_gather_context(run, p, C, context, ctx);
+    h->launches++;
+  }
+  if (z_init) {
+    e = cudaMemcpyAsync(z, z_init, N * ld * 4, cudaMemcpyDeviceToDevice, run);
+    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "z_init copy: %s", cudaGetErrorString(e));
+  } else {
+    launch_step_philox(run, p, h->d, 2, nullptr, nullptr, nullptr, nullptr, nullptr, seed, 0, nullptr, z);
+    h->launches++;
+  }
+
+  // one reverse step, captured once and replayed T times; it reads the step, the seed and the first draw index from the
+  // device, and the coefficient table at a fixed address.  The key holds every device address the captured step bakes in
+  // (the chain buffers, the plan, the workspace, the weights and their tensor-core streams) next to the plan and weights
+  // epochs, so a buffer that moved for any reason forces a new capture instead of a replay through a freed pointer.
+  float* eps = static_cast<float*>(h->eps_buf.p);
+  auto addr = [](const void* q) { return (long long)(uintptr_t)q; };
+  const std::vector<long long> key = {N, B, h->plan_epoch, h->weights_epoch, addr(h->smp_buf.p), addr(h->eps_buf.p),
+                                      addr(h->work_buf.p), addr(h->plan_buf.p), addr(h->rc_buf.p), addr(h->sched_buf.p),
+                                      addr(h->wbuf), addr(h->tc_blob.p), addr(h->tc_node_blob.p), addr(h->layers_dev.p)};
+  if (!h->smp_graph || key != h->smp_graph_key) {
+    if (h->smp_graph) cudaGraphExecDestroy(h->smp_graph);
+    h->smp_graph = nullptr;
+    h->smp_graph_key.clear();
+    const int64_t before = h->launches;
+    cudaGraph_t g = nullptr;
+    e = cudaStreamBeginCapture(run, cudaStreamCaptureModeThreadLocal);
+    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample capture: %s", cudaGetErrorString(e));
+    int32_t rc = forward_impl(h, run, z, nullptr, coef, ctr, ctx, eps);
+    if (rc == BDIFF_OK) {
+      launch_step_philox(run, p, h->d, 0, z, eps, coef, ctr, ctr + 1, 0, 0, seed_draw, z);
+      h->launches++;
+    }
+    e = cudaStreamEndCapture(run, &g);
+    h->smp_step_launches = h->launches - before;
+    h->launches = before;
+    if (rc != BDIFF_OK) { if (g) cudaGraphDestroy(g); return rc; }
+    if (e == cudaSuccess) e = cudaGraphInstantiate(&h->smp_graph, g, 0);
+    if (g) cudaGraphDestroy(g);
+    if (e != cudaSuccess) { h->smp_graph = nullptr; return h->fail(BDIFF_ECUDA, "sample graph: %s", cudaGetErrorString(e)); }
+    h->smp_graph_key = key;
+    h->smp_graph_builds++;
+  }
+  for (int r = 0; r < T && e == cudaSuccess; ++r) {
+    e = cudaGraphLaunch(h->smp_graph, run);
+    h->launches += h->smp_step_launches;
+  }
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample replay: %s", cudaGetErrorString(e));
+
+  // p(x, h | z_0) with draws draw0 + 2T, draw0 + 2T + 1, then the discretising tail of mol_gen_sample
+  int32_t rc = forward_impl(h, run, z, nullptr, dec, nullptr, ctx, eps);
+  if (rc != BDIFF_OK) return rc;
+  launch_step_philox(run, p, h->d, 1, z, eps, dec, nullptr, nullptr, seed, draw0 + 2ull * T, nullptr, xhn);
+  launch_sample_finish(run, p, h->d, h->scfg.num_atom_types, h->scfg.norm_values, h->scfg.norm_biases, xhn, xh, tot);
+  h->launches += 3;
+  if (batch_index) {
+    e = cudaMemcpyAsync(batch_index, bi_dev, N * 8, cudaMemcpyDeviceToDevice, run);
+    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "batch_index copy: %s", cudaGetErrorString(e));
+  }
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample: %s", cudaGetErrorString(e));
+  return bdiff_check(h, run);
+}
 
 }  // extern "C"

@@ -91,6 +91,20 @@ struct bdiff_handle {
   cudaStream_t side = nullptr;          // fork/join stream: the edge embedding runs next to the node embedding
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
 
+  // bdiff_sample: sampling constants, the chain's buffers, and the captured reverse step with the key it was built for
+  int weights_epoch = 0;                // bumped by every bdiff_set_weight
+  bool have_sample_cfg = false;
+  bdiff_sample_config scfg{};
+  DevBuf smp_buf;                       // batch_index, mask, z, decoded xh, ctx, coef table, decode row, counters, CoG sums
+  std::vector<int32_t> smp_counts;      // the batch of the handle's plan when bdiff_sample built it ...
+  int smp_plan_epoch = -1;              // ... and the plan epoch that plan got
+  cudaStream_t smp_stream = nullptr;    // the chain runs here when the caller passes the legacy stream (not capturable)
+  cudaEvent_t smp_ev = nullptr;
+  cudaGraphExec_t smp_graph = nullptr;
+  std::vector<long long> smp_graph_key;
+  int64_t smp_step_launches = 0;        // kernels in one captured reverse step
+  int64_t smp_graph_builds = 0;
+
   int fail(int code, const char* fmt, ...) {
     char buf[512];
     va_list ap;

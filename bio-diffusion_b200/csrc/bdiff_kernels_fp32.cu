@@ -6,6 +6,7 @@
 // gcpnet.py:1054-1066.  Reference citations are relative to /root/reference/src/.
 #include "bdiff_common.cuh"
 #include "bdiff_kernels.h"
+#include "bdiff_philox.cuh"
 
 namespace bdiff {
 
@@ -924,6 +925,150 @@ __global__ void __launch_bounds__(128) k_repaint_combine(Plan p, Dims d, float* 
   }
 }
 
+// ------------------------------------------------------------------------------- native chain (bdiff_sample)
+// k_step with the noise computed in place: noise_x = draw dx, noise_h = draw dx + 1 of `seed` (bdiff_philox.cuh), where
+// dx = draw0 + 2 * *step_ptr in mode 0 and draw0 otherwise ({seed, draw0} = seed_draw[0..1] when seed_draw is given).  Masking, centring and every arithmetic step are k_step's.
+// Mode 0 also advances the step counter: the last CTA to finish (all CTAs have read it by then) adds 1 and re-arms `done`.
+__global__ void __launch_bounds__(128) k_step_philox(Plan p, Dims d, int mode, const float* __restrict__ z,
+                                                     const float* __restrict__ eps, const float* __restrict__ coef_table,
+                                                     int* step_ptr, int* done, unsigned long long seed,
+                                                     unsigned long long draw0, const unsigned long long* seed_draw,
+                                                     float* __restrict__ out) {
+  const int step = step_ptr ? *step_ptr : 0;
+  if (seed_draw) {            // a captured step reads {seed, draw0} from the device, so one graph serves every seed
+    seed = seed_draw[0];
+    draw0 = seed_draw[1];
+  }
+  const float* coef = coef_table ? coef_table + 4 * step : nullptr;
+  const unsigned long long dx = draw0 + (mode == 0 ? 2ull * (unsigned)step : 0ull), dh = dx + 1;
+  __shared__ float red[4][4];
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const int ld = 3 + d.F;
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float m = p.mask[i] ? 1.f : 0.f;
+    s[0] += philox_normal(seed, dx, (unsigned long long)i * 3 + 0) * m;
+    s[1] += philox_normal(seed, dx, (unsigned long long)i * 3 + 1) * m;
+    s[2] += philox_normal(seed, dx, (unsigned long long)i * 3 + 2) * m;
+    s[3] += m;
+  }
+  block_sum4(s, red);
+  const float cnt = s[3];
+  const float ncx = cnt > 0.f ? s[0] / cnt : 0.f, ncy = cnt > 0.f ? s[1] / cnt : 0.f,
+              ncz = cnt > 0.f ? s[2] / cnt : 0.f;
+  const float c0 = mode == 2 ? 0.f : __ldg(coef + 0), c1 = mode == 2 ? 0.f : __ldg(coef + 1),
+              c2 = mode == 2 ? 1.f : __ldg(coef + 2);
+  float t[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float m = p.mask[i] ? 1.f : 0.f;
+    const float nc[3] = {ncx, ncy, ncz};
+    for (int c = 0; c < ld; ++c) {
+      float nz = (c < 3 ? philox_normal(seed, dx, (unsigned long long)i * 3 + c)
+                        : philox_normal(seed, dh, (unsigned long long)i * d.F + (c - 3))) * m;
+      if (c < 3) nz -= nc[c] * m;
+      float v;
+      if (mode == 0) v = z[(size_t)i * ld + c] / c0 - c1 * eps[(size_t)i * ld + c] + c2 * nz;
+      else if (mode == 1) v = c0 * (z[(size_t)i * ld + c] - c1 * eps[(size_t)i * ld + c]) + c2 * nz;
+      else v = nz;
+      out[(size_t)i * ld + c] = v;
+      if (c < 3) t[c] += v;
+    }
+  }
+  if (mode != 0) return;
+  block_sum4(t, red);
+  const float zx = cnt > 0.f ? t[0] / cnt : 0.f, zy = cnt > 0.f ? t[1] / cnt : 0.f, zz = cnt > 0.f ? t[2] / cnt : 0.f;
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float m = p.mask[i] ? 1.f : 0.f;
+    out[(size_t)i * ld + 0] -= zx * m;
+    out[(size_t)i * ld + 1] -= zy * m;
+    out[(size_t)i * ld + 2] -= zz * m;
+  }
+  if (!step_ptr) return;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(done, 1) == (int)gridDim.x - 1) {
+      *done = 0;
+      *step_ptr = step + 1;
+    }
+  }
+}
+
+__global__ void k_noise_fill(unsigned long long seed, unsigned long long draw, long long n, float* __restrict__ out) {
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < n) out[e] = philox_normal(seed, draw, (unsigned long long)e);
+}
+
+__global__ void k_philox_fill(unsigned long long seed, unsigned long long draw, long long blocks, uint32_t* __restrict__ out) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= blocks) return;
+  const Philox4 r = philox_block(seed, draw, (unsigned long long)b);
+  reinterpret_cast<uint4*>(out)[b] = make_uint4(r.w[0], r.w[1], r.w[2], r.w[3]);
+}
+
+// ctx[n, :] = context[molecule of n, :] (sampler.py's context[batch_index] * node_mask, every atom present)
+__global__ void k_gather_context(Plan p, int C, const float* __restrict__ context, float* __restrict__ ctx) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (long long)p.N * C) return;
+  const int n = (int)(g / C), c = (int)(g - (long long)n * C);
+  ctx[g] = context[(size_t)p.node_mol[n] * C + c];
+}
+
+// One CTA per molecule: the unnormalise / discretise tail of mol_gen_sample (sampler.py _finish, variational_diffusion.py
+// :892-907): x = xh.x * nv0; one_hot = argmax of (xh.h_cat * nv1 + nb1) (first maximum, NaN counts as the maximum);
+// charge = round-half-even(xh.h_int * nv2 + nb2) through int64.  Writes tot[k] = the molecule's coordinate sums.
+__global__ void __launch_bounds__(128) k_sample_finish(Plan p, Dims d, int A, float nv0, float nv1, float nb1, float nv2,
+                                                       float nb2, const float* __restrict__ xhn, float* __restrict__ out,
+                                                       float* __restrict__ tot) {
+  __shared__ float red[4][4];
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const int ld = 3 + d.F;
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float* row = xhn + (size_t)i * ld;
+    float* o = out + (size_t)i * ld;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      o[c] = __fmul_rn(row[c], nv0);
+      s[c] += o[c];
+    }
+    int best = 0;
+    float bv = 0.f;
+    for (int a = 0; a < A; ++a) {
+      const float v = __fadd_rn(__fmul_rn(row[3 + a], nv1), nb1);
+      if (a == 0 || (!(bv != bv) && (v > bv || v != v))) { best = a; bv = v; }
+    }
+    for (int a = 0; a < A; ++a) o[3 + a] = a == best ? 1.f : 0.f;
+    if (ld > 3 + A) o[3 + A] = (float)(long long)rintf(__fadd_rn(__fmul_rn(row[3 + A], nv2), nb2));
+  }
+  block_sum4(s, red);
+  if (threadIdx.x == 0) {
+    tot[3 * k + 0] = s[0];
+    tot[3 * k + 1] = s[1];
+    tot[3 * k + 2] = s[2];
+  }
+}
+
+// CoG drift fix (variational_diffusion.py:1391-1402): when max |tot| over the batch exceeds 5e-2, x -= tot[k] / n_k.
+__global__ void __launch_bounds__(128) k_sample_cog_fix(Plan p, Dims d, const float* __restrict__ tot, float* __restrict__ out) {
+  __shared__ int fire;
+  if (threadIdx.x == 0) fire = 0;
+  __syncthreads();
+  for (int j = threadIdx.x; j < 3 * p.B; j += 128)
+    if (fabsf(tot[j]) > 5e-2f) fire = 1;
+  __syncthreads();
+  if (!fire) return;
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const float cnt = (float)(n1 - n0);
+  const int ld = 3 + d.F;
+  for (int i = n0 + threadIdx.x; i < n1; i += 128)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[(size_t)i * ld + c] = __fsub_rn(out[(size_t)i * ld + c], __fdiv_rn(tot[3 * k + c], cnt));
+}
+
 // edge_index int64 [2, E] from the plan (gcpnet.py:1054-1066) — only when a caller asks for it.
 __global__ void k_edge_index(Plan p, long long* __restrict__ out) {
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1020,6 +1165,26 @@ void launch_repaint_combine(cudaStream_t st, const Plan& p, const Dims& d, float
                             const uint8_t* fixed, const float* noise_x, const float* noise_h,
                             const float* known_table, const int* op_ptr) {
   k_repaint_combine<<<p.B, 128, 0, st>>>(p, d, z, xh0, fixed, noise_x, noise_h, known_table, op_ptr);
+}
+void launch_step_philox(cudaStream_t st, const Plan& p, const Dims& d, int mode, const float* z, const float* eps,
+                        const float* coef_table, int* step_ptr, int* done, unsigned long long seed,
+                        unsigned long long draw0, const unsigned long long* seed_draw, float* out) {
+  k_step_philox<<<p.B, 128, 0, st>>>(p, d, mode, z, eps, coef_table, step_ptr, done, seed, draw0, seed_draw, out);
+}
+void launch_noise_fill(cudaStream_t st, unsigned long long seed, unsigned long long draw, long long n, float* out) {
+  if (n > 0) k_noise_fill<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seed, draw, n, out);
+}
+void launch_philox_fill(cudaStream_t st, unsigned long long seed, unsigned long long draw, long long blocks, uint32_t* out) {
+  if (blocks > 0) k_philox_fill<<<(unsigned)((blocks + 255) / 256), 256, 0, st>>>(seed, draw, blocks, out);
+}
+void launch_gather_context(cudaStream_t st, const Plan& p, int C, const float* context, float* ctx) {
+  const long long n = (long long)p.N * C;
+  if (n > 0) k_gather_context<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, C, context, ctx);
+}
+void launch_sample_finish(cudaStream_t st, const Plan& p, const Dims& d, int A, const float* nv, const float* nb,
+                          const float* xhn, float* out, float* tot) {
+  k_sample_finish<<<p.B, 128, 0, st>>>(p, d, A, nv[0], nv[1], nb[1], nv[2], nb[2], xhn, out, tot);
+  k_sample_cog_fix<<<p.B, 128, 0, st>>>(p, d, tot, out);
 }
 void launch_edge_index(cudaStream_t st, const Plan& p, long long* out) {
   if (p.E > 0) k_edge_index<<<(unsigned)((p.E + 255) / 256), 256, 0, st>>>(p, out);

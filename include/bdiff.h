@@ -169,6 +169,71 @@ BDIFF_API int32_t bdiff_renoise(bdiff_handle* h, void* stream, float* z, const f
  * error (BDIFF_ECUDA), never expected.  Call after a chain of bdiff_reverse_step / before trusting a result. */
 BDIFF_API int32_t bdiff_check(bdiff_handle* h, void* stream);
 
+/* ---- sampling through the C ABI alone ---------------------------------------------------------------------------------
+ * Replaces: EquivariantVariationalDiffusion.mol_gen_sample (variational_diffusion.py:1280-1412) as one call, for hosts
+ * without torch.  Minimal sequence: bdiff_create -> bdiff_set_weight (every parameter) -> bdiff_prepare ->
+ * bdiff_sample_setup -> bdiff_sample (as often as wanted).
+ *
+ * Noise: counter-based Philox4x32-10 (key = seed, 10 rounds) with Box-Muller, computed inside the step kernels; no
+ * generator state.  A chain is a sequence of "draws": buffer fills of N(0, I) values in the order the reference draws
+ * them — z_T as draws 0 (x, [N,3]) and 1 (h, [N,F]); reverse step r as draws 2+2r (x) and 3+2r (h); the decode as draws
+ * 2+2T and 3+2T.  A chain started from z_init has no z_T draws: everything moves down by 2.  Element e (row-major) of
+ * draw d is normal[e & 3] of block (counter = {e >> 2 (64 bit), d (64 bit)}, key = {seed lo, seed hi}): words (w0, w1)
+ * give normals 0 and 1, (w2, w3) normals 2 and 3, as r*cos and r*sin of r = sqrt(-2 ln((w_even + 0.5) 2^-32)),
+ * angle = 2 pi (w_odd 2^-32), evaluated in double and rounded to float.  The result is a pure function of (seed, d, e).
+ * The same seed and batch give bit-identical molecules; the same seed on a different batch composition does not
+ * reproduce a molecule (the CoG fix and molecule-boundary effects of the denoiser depend on the whole batch). */
+
+/* The model's sampling constants beyond bdiff_config: num_h must equal num_atom_types + include_charges. */
+typedef struct bdiff_sample_config {
+  int32_t num_atom_types;    /* A: one-hot columns of h                                                            */
+  int32_t include_charges;   /* 0 / 1: h ends with one charge column                                               */
+  int32_t model_timesteps;   /* T of the model's gamma table (diffusion_cfg.num_timesteps; 1000 shipped)           */
+  int32_t reserved;          /* 0                                                                                  */
+  double schedule_power;     /* noise_schedule polynomial_<power> (2 shipped)                                      */
+  double noise_precision;    /* diffusion_cfg.noise_precision (1e-5 shipped)                                       */
+  float norm_values[3];      /* diffusion_cfg.norm_values: x, one-hot, charges                                     */
+  float norm_biases[3];      /* diffusion_cfg.norm_biases; [0] is unused (the reference's None)                    */
+} bdiff_sample_config;
+
+/* Host only (no GPU needed): the tables the chain reads, for a chain of num_timesteps steps.  coef_out[num_timesteps*4]
+ * receives rows {alpha_ts, c_eps, sigma, t} of reverse steps s = num_timesteps-1 .. 0 (bdiff_reverse_step's table),
+ * decode_out[4] = {1/alpha_0, sigma_0, sigma_x, 0} (bdiff_decode_z0's).  gamma is built in fp64 like the reference's
+ * PredefinedNoiseSchedule and rounded to fp32 (bit-equal to bdiff/schedule.py's); each coefficient is then evaluated in
+ * fp64 from those fp32 gamma values and rounded once, so the tables do not depend on a vector math library or on the
+ * CPU.  bdiff/schedule.py evaluates the same formulas in fp32 with torch's CPU kernels, whose result varies with the
+ * machine (MKL's exp, SLEEF and the SIMD width torch dispatches to); its c_eps and sigma differ from these by up to
+ * ~5e-5 relative at 1000 steps.  To rerun a chain on tables computed elsewhere, pass them to bdiff_sample. */
+BDIFF_API int32_t bdiff_schedule_tables(const bdiff_sample_config* cfg, int32_t num_timesteps, float* coef_out,
+                                        float* decode_out);
+
+/* Stores the sampling constants on the handle (required before bdiff_sample). */
+BDIFF_API int32_t bdiff_sample_setup(bdiff_handle* h, const bdiff_sample_config* cfg);
+
+/* out fp32[rows*cols] (device) <- draw `draw_index` of `seed`: the values the sampling kernels compute internally. */
+BDIFF_API int32_t bdiff_noise_fill(void* stream, uint64_t seed, uint64_t draw_index, int64_t rows, int64_t cols,
+                                   float* out);
+/* out uint32[4*blocks] (device) <- the raw Philox4x32-10 words of blocks 0 .. blocks-1 of draw `draw_index`. */
+BDIFF_API int32_t bdiff_philox_fill(void* stream, uint64_t seed, uint64_t draw_index, int64_t blocks, uint32_t* out);
+
+/* The whole chain: z_T (or z_init), num_timesteps reverse steps replayed from one captured CUDA graph (cached on the
+ * handle; rebuilt when the batch, the plan or the weights change), the decode, then what mol_gen_sample does last
+ * (:1388-1402): argmax one-hot, rounded charges, and the CoG drift fix when the largest per-molecule coordinate sum
+ * exceeds 5e-2.  Ends with bdiff_check (synchronises `stream`).
+ *   num_nodes_host int32[num_mols] (host) atoms per molecule, all >= 1; no padding mask (every atom is present)
+ *   context        fp32[num_mols, num_context] (device), required iff num_context > 0
+ *   z_init         fp32[N, 3+num_h] (device, normalised, CoG-free) or NULL; z_init_shape = {N, 3+num_h} (host)
+ *   tables_host    NULL (bdiff_schedule_tables) or num_timesteps*4 + 4 floats (host): coef rows then the decode row, to
+ *                  run on tables computed elsewhere (bdiff/sampler.py passes its own, so that its chains and this one
+ *                  are bit-identical)
+ *   xh             fp32[N, 3+num_h] (device) <- [x | one_hot | charges]; batch_index int64[N] (device) or NULL
+ * Replans the topology (one D2H + H2D) only when the batch differs from the last call's or another plan intervened. */
+BDIFF_API int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host,
+                               const float* context, int32_t num_timesteps, uint64_t seed, const float* z_init,
+                               const int64_t* z_init_shape, const float* tables_host, float* xh, int64_t* batch_index);
+/* Number of reverse-step graphs bdiff_sample has captured on this handle (cache diagnostics). */
+BDIFF_API int64_t bdiff_sample_graph_builds(const bdiff_handle* h);
+
 /* ---- optimiser side of a training step (SURVEY.md §8 a21): adaptive gradient-norm clipping + AdamW(amsgrad) + EMA --
  * Replaces, per step: get_grad_norm + Queue statistics + clip_gradients (qm9_mol_gen_ddpm.py:1267-1304,
  * src/models/__init__.py:90-113,442-466), torch.optim.AdamW(lr 1e-4, weight_decay 1e-12, amsgrad) (configs/model/

@@ -68,7 +68,15 @@ PROTOTYPES = {
     "bdiff_philox_fill": (C.c_int32, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_void_p]),
     "bdiff_sample": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
                                  C.c_uint64, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bdiff_sample_frames": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
+                                        C.c_uint64, C.c_void_p, C.POINTER(C.c_int64), C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
     "bdiff_sample_graph_builds": (C.c_int64, [C.c_void_p]),
+    "bdiff_repaint_tables": (C.c_int32, [C.POINTER(SampleConfig)] + [C.c_int32] * 4 + [C.c_void_p] * 12),
+    "bdiff_inpaint": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p, C.c_int32,
+                                  C.c_int32, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                  C.c_void_p, C.c_void_p]),
+    "bdiff_inpaint_graph_builds": (C.c_int64, [C.c_void_p]),
     "bdiff_check_stability": (C.c_int32, [C.c_void_p] * 4 + [C.c_int32, C.c_int32] + [C.c_void_p] * 3 + [C.c_float] * 3 +
                               [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bdiff_bond_orders": (C.c_int32, [C.c_void_p] * 5 + [C.c_int32, C.c_int32] + [C.c_void_p] * 3 + [C.c_float] * 3 +

@@ -82,3 +82,28 @@ def schedule_tables(cfg: DenoiserConfig, num_timesteps: int) -> Tuple[torch.Tens
     if rc != 0:
         raise _lib.BdiffError(f"bdiff_schedule_tables failed (code {rc})")
     return coef, dec
+
+
+def repaint_tables(cfg: DenoiserConfig, num_timesteps: int, num_resamplings: int, jump_length: int,
+                   return_frames: int = 1) -> dict:
+    """The library's RePaint program (bdiff_repaint_tables; no GPU needed), with the keys of schedule.repaint_program:
+    rev [ops, 4], known [ops, 2], jump [jumps, 4], decode [4], s_of_op / slot / jump_after [ops], num_jumps, and the first
+    draw of each op (op_draw [ops]), jump (jump_draw [jumps]) and of the decode (decode_draw)."""
+    sc = sample_config(cfg)
+    lib = _lib.load()
+    args = (C.byref(sc), int(num_timesteps), int(num_resamplings), int(jump_length), int(return_frames))
+    ops, jumps = C.c_int32(0), C.c_int32(0)
+    if lib.bdiff_repaint_tables(*args, C.byref(ops), C.byref(jumps), *([None] * 10)) != 0:
+        raise _lib.BdiffError("bdiff_repaint_tables refused its arguments")
+    o, j = ops.value, jumps.value
+    t = dict(rev=torch.empty((o, 4)), known=torch.empty((o, 2)), jump=torch.empty((j, 4)), decode=torch.empty(4),
+             s_of_op=torch.empty(o, dtype=torch.int32), slot=torch.empty(o, dtype=torch.int32),
+             jump_after=torch.empty(o, dtype=torch.uint8), op_draw=torch.empty(o, dtype=torch.int64),
+             jump_draw=torch.empty(j, dtype=torch.int64))
+    dd = C.c_uint64(0)
+    ptrs = [C.c_void_p(t[k].data_ptr()) for k in ("rev", "known", "jump", "decode", "s_of_op", "slot", "jump_after",
+                                                  "op_draw", "jump_draw")]
+    if lib.bdiff_repaint_tables(*args, C.byref(ops), C.byref(jumps), *ptrs, C.byref(dd)) != 0:
+        raise _lib.BdiffError("bdiff_repaint_tables failed")
+    t.update(num_jumps=j, decode_draw=dd.value, jump_after=t["jump_after"].bool())
+    return t

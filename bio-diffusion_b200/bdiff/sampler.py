@@ -252,17 +252,17 @@ class GCDMSampler:
         return_frames = F > 1, out is [F, N, 3+A(+1)]: frame k is the unnormalised latent after the step that lands on
         s = k*T/F, frame 0 the decoded molecules (no CoG drift correction, as in the reference).
 
-        `seed` = s runs the whole chain in the library instead (bdiff_sample): the noise is drawn inside the step kernels
-        from Philox4x32-10 keyed by s, so nothing is drawn from torch's generator.  The result is bit-identical to
-        `sample(..., noise=philox_noise(s))` and is reproducible from the seed and the batch.  Not combinable with
-        `noise`, `node_mask`, `return_z0`, `record_moments` or `return_frames` > 1.
+        `seed` = s runs the whole chain in the library instead (bdiff_sample_frames): the noise is drawn inside the step
+        kernels from Philox4x32-10 keyed by s, so nothing is drawn from torch's generator.  The result, frames included, is
+        bit-identical to `sample(..., noise=philox_noise(s))` and is reproducible from the seed and the batch.  Not
+        combinable with `noise`, `node_mask`, `return_z0` or `record_moments`.
         """
         steps = self.cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
         if seed is not None:
-            if noise is not None or node_mask is not None or return_z0 or record_moments or return_frames != 1:
-                raise ValueError("sample(seed=...) runs the native chain: noise, node_mask, return_z0, record_moments and "
-                                 "return_frames > 1 are not available there")
-            return self._sample_native(num_nodes, context, steps, int(seed), z_init)
+            if noise is not None or node_mask is not None or return_z0 or record_moments:
+                raise ValueError("sample(seed=...) runs the native chain: noise, node_mask, return_z0 and record_moments "
+                                 "are not available there")
+            return self._sample_native(num_nodes, context, steps, int(seed), z_init, int(return_frames))
         check_frames(steps, return_frames)
         dev = self._device()
         num_nodes = num_nodes.to(dev, non_blocking=True)
@@ -277,47 +277,57 @@ class GCDMSampler:
         self.last_moments = st["moments"].clone() if record_moments else None
         return (out, batch_index, mask, st["z"].clone()) if return_z0 else (out, batch_index, mask)
 
-    def _sample_native(self, num_nodes: torch.Tensor, context: Optional[torch.Tensor], steps: int, seed: int,
-                       z_init: Optional[torch.Tensor]):
-        """sample(seed=...): one bdiff_sample call on this sampler's coefficient tables."""
+    def _native_setup(self, b: int, context: Optional[torch.Tensor]):
+        """What a native chain needs before its call: the device, the context on it, weights and sampling constants."""
         cfg = self.cfg
         dev = self._device()
         if dev.type != "cuda":
             raise _lib.BdiffError("GCDMSampler needs the denoiser on a CUDA device (no CPU fallback)")
-        if steps < 1:
-            raise ValueError(f"num_timesteps must be >= 1, got {steps}")
-        counts = num_nodes.detach().reshape(-1).to("cpu", torch.int32).contiguous()
-        b, n = int(counts.shape[0]), int(counts.sum())
         if cfg.num_context:
             if context is None or tuple(context.shape) != (b, cfg.num_context):
                 raise ValueError(f"property-conditional configuration: `context` [{b}, {cfg.num_context}] is required")
             context = context.to(dev, torch.float32).contiguous()
         elif context is not None:
             raise ValueError("`context` given to a configuration without conditioning")
+        self.net.sync_weights()
+        _lib.check(self.net._handle, _lib.load().bdiff_sample_setup(self.net._handle, C.byref(sample_config(cfg))),
+                   "bdiff_sample_setup")
+        return dev, context
+
+    def _native_call(self, name: str, *args) -> None:
+        """Runs one native chain; the library plans the batch itself, so the module's plan cache and the graphs captured
+        on it are stale afterwards."""
+        lib = _lib.load()
+        h = self.net._handle
+        before = lib.bdiff_launch_count(h)
+        self.net._plan_key = None
+        self.net._plan_epoch += 1
+        _lib.check(h, getattr(lib, name)(h, self.net._stream(), *args), name)
+        self.kernel_launches += int(lib.bdiff_launch_count(h) - before)
+
+    def _sample_native(self, num_nodes: torch.Tensor, context: Optional[torch.Tensor], steps: int, seed: int,
+                       z_init: Optional[torch.Tensor], frames: int):
+        """sample(seed=...): one bdiff_sample_frames call on this sampler's coefficient tables."""
+        cfg = self.cfg
+        if steps < 1:
+            raise ValueError(f"num_timesteps must be >= 1, got {steps}")
+        check_frames(steps, frames)
+        counts = num_nodes.detach().reshape(-1).to("cpu", torch.int32).contiguous()
+        b, n = int(counts.shape[0]), int(counts.sum())
+        dev, context = self._native_setup(b, context)
         zi = None
         zshape = None
         if z_init is not None:
             zi = z_init.to(dev, torch.float32).contiguous()
             zshape = (C.c_int64 * 2)(*zi.shape) if zi.dim() == 2 else (C.c_int64 * 2)(-1, -1)
-        self.net.sync_weights()
-        lib = _lib.load()
-        h = self.net._handle
-        sc = sample_config(cfg)
-        _lib.check(h, lib.bdiff_sample_setup(h, C.byref(sc)), "bdiff_sample_setup")
         # the Python chain's own tables, so that both chains run the same coefficients bit for bit
         tables = torch.cat((step_coefficient_table(self.gamma, steps).reshape(-1), decode_coefficients(self.gamma)))
         tables = tables.to(torch.float32).contiguous()
-        out = torch.empty((n, 3 + cfg.num_h), dtype=torch.float32, device=dev)
+        out = torch.empty(((frames,) if frames > 1 else ()) + (n, 3 + cfg.num_h), dtype=torch.float32, device=dev)
         bi = torch.empty(n, dtype=torch.int64, device=dev)
-        before = lib.bdiff_launch_count(h)
-        # the library plans this batch itself: the module's plan cache and the graphs captured on it are stale after it
-        self.net._plan_key = None
-        self.net._plan_epoch += 1
-        rc = lib.bdiff_sample(h, self.net._stream(), b, counts.numpy().ctypes.data_as(C.POINTER(C.c_int32)), _ptr(context),
-                              steps, seed & 0xFFFFFFFFFFFFFFFF, _ptr(zi), zshape, C.c_void_p(tables.data_ptr()),
-                              _ptr(out), _ptr(bi))
-        _lib.check(h, rc, "bdiff_sample")
-        self.kernel_launches += int(lib.bdiff_launch_count(h) - before)
+        self._native_call("bdiff_sample_frames", b, counts.numpy().ctypes.data_as(C.POINTER(C.c_int32)), _ptr(context),
+                          steps, seed & 0xFFFFFFFFFFFFFFFF, _ptr(zi), zshape, frames, C.c_void_p(tables.data_ptr()),
+                          _ptr(out), _ptr(bi))
         return out, bi, torch.ones(n, dtype=torch.bool, device=dev)
 
     def nan_guard_count(self, reset: bool = False) -> int:
@@ -420,10 +430,22 @@ class GCDMSampler:
             raise ValueError("`context` given to a configuration without conditioning")
         return num_nodes, batch_index, parts, node_mask_fixed.bool(), context
 
+    @staticmethod
+    def _center_on_fixed(xh0: torch.Tensor, batch_index: torch.Tensor, fixed: torch.Tensor, b: int) -> torch.Tensor:
+        """xh0 (host, float32) with x centred on the fixed atoms of its molecule (:1617-1633); a molecule without fixed
+        atoms is not moved.  Sequential float32 sums on the host like the reference, so run-to-run reproducible (the
+        device's index_add_ sums in atomic order)."""
+        xh0 = xh0.clone()
+        ff = fixed.float()
+        tot = torch.zeros((b, 3)).index_add_(0, batch_index, xh0[:, :3] * ff.unsqueeze(-1))
+        cnt = torch.zeros(b).index_add_(0, batch_index, ff)
+        xh0[:, :3] -= (tot / cnt.clamp(min=1.0).unsqueeze(-1))[batch_index]
+        return xh0
+
     @torch.inference_mode()
     def inpaint(self, molecule: dict, node_mask_fixed: torch.Tensor, num_resamplings: int = 1, jump_length: int = 1,
                 return_frames: int = 1, num_timesteps: Optional[int] = None, context: Optional[torch.Tensor] = None,
-                noise: Optional[NoiseFn] = None) -> torch.Tensor:
+                noise: Optional[NoiseFn] = None, seed: Optional[int] = None) -> torch.Tensor:
         """EquivariantVariationalDiffusion.inpaint (variational_diffusion.py:1580-1789): generate the rest of each molecule
         around the atoms with node_mask_fixed = True, which keep their type and 3-D position (RePaint).
 
@@ -434,11 +456,18 @@ class GCDMSampler:
         without fixed atoms is sampled freely.  `noise(shape)` optionally injects the randn draws in the reference's
         order: z_T, then per denoise op the known part and the unknown part, per jump one pair, the final decode.
         Returns out [N, 3+A(+1)], or [F, N, 3+A(+1)] for return_frames = F > 1 (frame 0 = the molecules).
+
+        `seed` = s runs the whole chain in the library instead (bdiff_inpaint), with the noise drawn inside its kernels;
+        bit-identical to `inpaint(..., noise=philox_noise(s))`.  Not combinable with `noise`.
         """
         steps = self.cfg.num_timesteps if num_timesteps is None else int(num_timesteps)
         r, j, nfr = int(num_resamplings), int(jump_length), int(return_frames)
         check_repaint(r, j, steps, nfr)
+        if seed is not None and noise is not None:
+            raise ValueError("inpaint(seed=...) runs the native chain: noise is not available there")
         num_nodes, batch_index, parts, fixed, context = self._inpaint_inputs(self.cfg, molecule, node_mask_fixed, context)
+        if seed is not None:
+            return self._inpaint_native(num_nodes, parts, fixed, context, steps, r, j, nfr, int(seed))
         dev = self._device()
         b = int(num_nodes.shape[0])
         n = int(batch_index.shape[0])
@@ -446,15 +475,25 @@ class GCDMSampler:
         mask = torch.ones(n, dtype=torch.bool, device=dev)          # inpaint has no padding mask (:1638)
         st, batch_index, mask = self._prepare(batch_index, mask, b, context, steps, (r, j), nfr)   # context: (:1614-1615)
 
-        # xh0 with x centred on the fixed atoms of its molecule (:1617-1633); a molecule without fixed atoms is not moved.
-        # A one-off step on the host: sequential float32 sums like the reference, and run-to-run reproducible (the
-        # device's index_add_ sums in atomic order)
         xh0 = torch.cat([p.detach().to("cpu", torch.float32).reshape(n, -1) for p in parts], dim=-1)
-        bi_h = batch_index.cpu()
-        ff = fixed.cpu().float()
-        tot = torch.zeros((b, 3)).index_add_(0, bi_h, xh0[:, :3] * ff.unsqueeze(-1))
-        cnt = torch.zeros(b).index_add_(0, bi_h, ff)
-        xh0[:, :3] -= (tot / cnt.clamp(min=1.0).unsqueeze(-1))[bi_h]
-        st["xh0"].copy_(xh0)
+        st["xh0"].copy_(self._center_on_fixed(xh0, batch_index.cpu(), fixed.cpu(), b))
         st["fixed"].copy_(fixed.cpu().to(torch.uint8))
         return self._chain(st, noise, batch_index, mask, b)
+
+    def _inpaint_native(self, num_nodes: torch.Tensor, parts, fixed: torch.Tensor, context: Optional[torch.Tensor],
+                        steps: int, r: int, j: int, frames: int, seed: int) -> torch.Tensor:
+        """inpaint(seed=...): one bdiff_inpaint call on this sampler's RePaint program (the tables the Python chain reads)."""
+        cfg = self.cfg
+        counts = num_nodes.to(torch.int32).contiguous()
+        b, n = int(counts.shape[0]), int(counts.sum())
+        dev, context = self._native_setup(b, context)
+        xh0 = torch.cat([p.detach().to("cpu", torch.float32).reshape(n, -1) for p in parts], dim=-1).contiguous()
+        fx = fixed.cpu().to(torch.uint8).contiguous()
+        prog = repaint_program(self.gamma, r, j, steps, frames)
+        tables = torch.cat((prog["rev"].reshape(-1), prog["known"].reshape(-1), prog["jump"][:prog["num_jumps"]].reshape(-1),
+                            decode_coefficients(self.gamma))).to(torch.float32).contiguous()
+        out = torch.empty(((frames,) if frames > 1 else ()) + (n, 3 + cfg.num_h), dtype=torch.float32, device=dev)
+        self._native_call("bdiff_inpaint", b, counts.numpy().ctypes.data_as(C.POINTER(C.c_int32)), _ptr(context), steps, r,
+                          j, seed & 0xFFFFFFFFFFFFFFFF, C.c_void_p(xh0.data_ptr()), C.c_void_p(fx.data_ptr()), frames,
+                          C.c_void_p(tables.data_ptr()), _ptr(out), None)
+        return out

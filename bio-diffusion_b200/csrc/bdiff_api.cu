@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
 #include <utility>
@@ -304,7 +305,11 @@ void bdiff_destroy(bdiff_handle* h) {
   if (h->smp_graph) cudaGraphExecDestroy(h->smp_graph);
   if (h->smp_ev) cudaEventDestroy(h->smp_ev);
   if (h->smp_stream) cudaStreamDestroy(h->smp_stream);
-  h->smp_buf.release();
+  if (h->inp_op_graph) cudaGraphExecDestroy(h->inp_op_graph);
+  if (h->inp_jump_graph) cudaGraphExecDestroy(h->inp_jump_graph);
+  h->smp_buf.release(); h->smp_slot.release(); h->smp_frames.release();
+  for (DevBuf* b : {&h->inp_buf, &h->inp_rev, &h->inp_known, &h->inp_slot, &h->inp_draw, &h->inp_jump, &h->inp_jdraw})
+    b->release();
   h->plan_buf.release(); h->rc_buf.release(); h->layers_dev.release(); h->sched_buf.release(); h->work_buf.release(); h->eps_buf.release(); h->tu_buf.release(); h->tc_blob.release(); h->tc_node_blob.release(); h->stage_buf.release(); h->jobs_dev.release();
   delete h;
 }
@@ -738,35 +743,123 @@ int32_t bdiff_philox_fill(void* stream, uint64_t seed, uint64_t draw_index, int6
 }
 
 int64_t bdiff_sample_graph_builds(const bdiff_handle* h) { return h ? h->smp_graph_builds : 0; }
+int64_t bdiff_inpaint_graph_builds(const bdiff_handle* h) { return h ? h->inp_graph_builds : 0; }
+
+// The stream a native chain runs on: the caller's, or, for the legacy default stream (which cannot be captured), the
+// handle's own stream ordered after it.
+static int32_t chain_stream(bdiff_handle* h, void* stream, cudaStream_t* run) {
+  *run = static_cast<cudaStream_t>(stream);
+  if (*run) return BDIFF_OK;
+  cudaError_t e = cudaSuccess;
+  if (!h->smp_stream) {
+    e = cudaStreamCreateWithFlags(&h->smp_stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->smp_ev, cudaEventDisableTiming);
+    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
+  }
+  *run = h->smp_stream;
+  e = cudaEventRecord(h->smp_ev, cudaStreamLegacy);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(*run, h->smp_ev, 0);
+  return e == cudaSuccess ? BDIFF_OK : h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
+}
+
+// Writes the batch's batch_index and mask into the chain's buffers (on every call: a grown buffer is a zeroed allocation
+// even when the plan is reused) and plans the topology when the batch changed or another plan replaced the chain's.
+static int32_t chain_batch(bdiff_handle* h, cudaStream_t run, const std::vector<int32_t>& counts, int64_t* bi_dev,
+                           uint8_t* mask_dev, std::vector<int32_t>* last_counts, int* last_epoch) {
+  std::vector<int64_t> bi;
+  for (size_t k = 0; k < counts.size(); ++k) bi.insert(bi.end(), (size_t)counts[k], (int64_t)k);
+  const long long N = (long long)bi.size();
+  cudaError_t e = cudaMemcpyAsync(bi_dev, bi.data(), N * 8, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemsetAsync(mask_dev, 1, N, run);
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample batch: %s", cudaGetErrorString(e));
+  if (h->have_plan && counts == *last_counts && h->plan_epoch == *last_epoch) return BDIFF_OK;
+  last_counts->clear();
+  int32_t rc = bdiff_plan_topology(h, run, (int32_t)counts.size(), N, bi_dev, mask_dev, nullptr);
+  if (rc != BDIFF_OK) return rc;
+  *last_counts = counts;
+  *last_epoch = h->plan_epoch;
+  return BDIFF_OK;
+}
+
+// What every captured chain body bakes in besides its own buffers: the plan, the workspace, the weights and their
+// tensor-core streams, next to the plan and weights epochs.  A buffer that moved for any reason changes the key, so it
+// forces a new capture instead of a replay through a freed pointer.
+static std::vector<long long> chain_key(const bdiff_handle* h, std::initializer_list<long long> own) {
+  auto addr = [](const void* q) { return (long long)(uintptr_t)q; };
+  std::vector<long long> key = {h->plan_epoch, h->weights_epoch, addr(h->eps_buf.p), addr(h->work_buf.p),
+                                addr(h->plan_buf.p), addr(h->rc_buf.p), addr(h->sched_buf.p), addr(h->wbuf),
+                                addr(h->tc_blob.p), addr(h->tc_node_blob.p), addr(h->layers_dev.p)};
+  key.insert(key.end(), own);
+  return key;
+}
+
+// Captures body() on `run` into *graph (replacing the old one); *launches receives the kernels one replay runs.
+static int32_t chain_capture(bdiff_handle* h, cudaStream_t run, const std::function<int32_t()>& body,
+                             cudaGraphExec_t* graph, int64_t* launches) {
+  if (*graph) cudaGraphExecDestroy(*graph);
+  *graph = nullptr;
+  const int64_t before = h->launches;
+  cudaGraph_t g = nullptr;
+  cudaError_t e = cudaStreamBeginCapture(run, cudaStreamCaptureModeThreadLocal);
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "chain capture: %s", cudaGetErrorString(e));
+  const int32_t rc = body();
+  e = cudaStreamEndCapture(run, &g);
+  *launches = h->launches - before;
+  h->launches = before;
+  if (rc != BDIFF_OK) { if (g) cudaGraphDestroy(g); return rc; }
+  if (e == cudaSuccess) e = cudaGraphInstantiate(graph, g, 0);
+  if (g) cudaGraphDestroy(g);
+  if (e != cudaSuccess) { *graph = nullptr; return h->fail(BDIFF_ECUDA, "chain graph: %s", cudaGetErrorString(e)); }
+  return BDIFF_OK;
+}
+
+// p(x, h | z_0) with draws decode_draw and decode_draw + 1, the discretising tail of mol_gen_sample into out[0 .. N), and
+// for F > 1 frames 1 .. F-1 behind it; ends with bdiff_check.
+static int32_t chain_tail(bdiff_handle* h, cudaStream_t run, float* z, const float* ctx, const float* dec,
+                          unsigned long long seed, unsigned long long decode_draw, float* xhn, float* tot,
+                          const float* frames, int F, const int64_t* bi_dev, float* out, int64_t* batch_index) {
+  const Plan& p = h->plan;
+  const size_t rows = (size_t)p.N * (3 + h->d.F);
+  float* eps = static_cast<float*>(h->eps_buf.p);
+  int32_t rc = forward_impl(h, run, z, nullptr, dec, nullptr, ctx, eps);
+  if (rc != BDIFF_OK) return rc;
+  launch_step_philox(run, p, h->d, 1, z, eps, dec, nullptr, nullptr, seed, decode_draw, nullptr, nullptr, xhn);
+  launch_sample_finish(run, p, h->d, h->scfg.num_atom_types, h->scfg.norm_values, h->scfg.norm_biases, xhn, out, tot,
+                       F == 1);
+  h->launches += F == 1 ? 3 : 2;
+  cudaError_t e = cudaSuccess;
+  if (F > 1) e = cudaMemcpyAsync(out + rows, frames + rows, (F - 1) * rows * 4, cudaMemcpyDeviceToDevice, run);
+  if (e == cudaSuccess && batch_index) e = cudaMemcpyAsync(batch_index, bi_dev, p.N * 8, cudaMemcpyDeviceToDevice, run);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "chain tail: %s", cudaGetErrorString(e));
+  return bdiff_check(h, run);
+}
 
 int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host, const float* context,
                      int32_t num_timesteps, uint64_t seed, const float* z_init, const int64_t* z_init_shape,
                      const float* tables_host, float* xh, int64_t* batch_index) {
+  return bdiff_sample_frames(h, stream, num_mols, num_nodes_host, context, num_timesteps, seed, z_init, z_init_shape, 1,
+                             tables_host, xh, batch_index);
+}
+
+int32_t bdiff_sample_frames(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host,
+                            const float* context, int32_t num_timesteps, uint64_t seed, const float* z_init,
+                            const int64_t* z_init_shape, int32_t return_frames, const float* tables_host, float* out,
+                            int64_t* batch_index) {
   if (!h) return BDIFF_EINVAL;
   if (!h->have_sample_cfg) return h->fail(BDIFF_ESTATE, "bdiff_sample_setup has not been called");
-  const std::string why = sample_args_error(h->d.F, h->d.C, h->scfg, num_mols, num_nodes_host, context, num_timesteps,
-                                            z_init, z_init_shape, xh);
+  std::string why = sample_args_error(h->d.F, h->d.C, h->scfg, num_mols, num_nodes_host, context, num_timesteps,
+                                      z_init, z_init_shape, out);
+  if (why.empty()) why = frames_args_error(num_timesteps, return_frames);
   if (!why.empty()) return h->fail(BDIFF_EINVAL, "bdiff_sample: %s", why.c_str());
   if (bdiff_weights_missing(h) != 0) return h->fail(BDIFF_ESTATE, "%d parameters not set", bdiff_weights_missing(h));
-  const int B = num_mols, T = num_timesteps, F = h->d.F, C = h->d.C, ld = 3 + F;
+  const int B = num_mols, T = num_timesteps, F = return_frames, C = h->d.C, ld = 3 + h->d.F;
   std::vector<int32_t> counts(num_nodes_host, num_nodes_host + B);
   long long N = 0;
   for (int32_t c : counts) N += c;
-
-  // the legacy default stream cannot be captured: run on the handle's own stream, ordered after it
-  cudaStream_t run = static_cast<cudaStream_t>(stream);
-  cudaError_t e = cudaSuccess;
-  if (!run) {
-    if (!h->smp_stream) {
-      e = cudaStreamCreateWithFlags(&h->smp_stream, cudaStreamNonBlocking);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->smp_ev, cudaEventDisableTiming);
-      if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
-    }
-    run = h->smp_stream;
-    e = cudaEventRecord(h->smp_ev, cudaStreamLegacy);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(run, h->smp_ev, 0);
-    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample stream: %s", cudaGetErrorString(e));
-  }
+  cudaStream_t run;
+  int32_t rc = chain_stream(h, stream, &run);
+  if (rc != BDIFF_OK) return rc;
 
   // chain buffers: batch_index, mask, z, decoded xh, per-atom context, {step, done, seed, draw0}, CoG sums, decode row,
   // and last the coefficient table, so that no buffer the captured step reads moves with the chain length
@@ -775,7 +868,9 @@ int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int3
   const size_t o_bi = take(N * 8), o_mask = take(N), o_z = take(N * ld * 4), o_xhn = take(N * ld * 4),
                o_ctx = take(N * C * 4), o_ctr = take(24), o_tot = take((size_t)B * 12), o_dec = take(16),
                o_coef = take((size_t)T * 16);
-  e = h->smp_buf.ensure(at);
+  cudaError_t e = h->smp_buf.ensure(at);
+  if (e == cudaSuccess && F > 1) e = h->smp_slot.ensure((size_t)T * 4);
+  if (e == cudaSuccess && F > 1) e = h->smp_frames.ensure((size_t)(F + 1) * N * ld * 4);
   if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "sample buffers: %s", cudaGetErrorString(e));
   unsigned char* base = static_cast<unsigned char*>(h->smp_buf.p);
   int64_t* bi_dev = reinterpret_cast<int64_t*>(base + o_bi);
@@ -787,23 +882,11 @@ int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int3
   int* ctr = reinterpret_cast<int*>(base + o_ctr);                                   // {step, done}
   unsigned long long* seed_draw = reinterpret_cast<unsigned long long*>(base + o_ctr + 8);   // {seed, draw0}
   float* tot = reinterpret_cast<float*>(base + o_tot);
+  int* slot = static_cast<int*>(h->smp_slot.p);
+  float* frames = static_cast<float*>(h->smp_frames.p);
 
-  // batch_index and mask are written on every call: they live in smp_buf, which ensure() above may just have replaced
-  // with a zeroed allocation (a longer chain grows it) even when the plan below is reused
-  std::vector<int64_t> bi((size_t)N);
-  for (int k = 0, i = 0; k < B; ++k)
-    for (int j = 0; j < counts[k]; ++j) bi[i++] = k;
-  e = cudaMemcpyAsync(bi_dev, bi.data(), N * 8, cudaMemcpyHostToDevice, run);
-  if (e == cudaSuccess) e = cudaMemsetAsync(base + o_mask, 1, N, run);
-  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample batch: %s", cudaGetErrorString(e));
-  // topology: replanned only when the batch changed or another plan replaced ours
-  if (!h->have_plan || counts != h->smp_counts || h->plan_epoch != h->smp_plan_epoch) {
-    h->smp_counts.clear();
-    int32_t rc = bdiff_plan_topology(h, run, B, N, bi_dev, base + o_mask, nullptr);
-    if (rc != BDIFF_OK) return rc;
-    h->smp_counts = counts;
-    h->smp_plan_epoch = h->plan_epoch;
-  }
+  rc = chain_batch(h, run, counts, bi_dev, base + o_mask, &h->smp_counts, &h->smp_plan_epoch);
+  if (rc != BDIFF_OK) return rc;
 
   std::vector<float> tables((size_t)T * 4 + 4);
   if (tables_host) {
@@ -818,6 +901,15 @@ int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int3
   const unsigned long long draw0 = z_init ? 0 : 2, sd[2] = {seed, draw0};
   if (e == cudaSuccess) e = cudaMemsetAsync(ctr, 0, 8, run);
   if (e == cudaSuccess) e = cudaMemcpyAsync(seed_draw, sd, 16, cudaMemcpyHostToDevice, run);
+  std::vector<int32_t> slots;
+  if (F > 1) {            // reverse step r lands on s = T-1-r; the steps between frames write the dummy slot F
+    for (int r = 0; r < T; ++r) {
+      const int v = frame_slot(T - 1 - r, T, F);
+      slots.push_back(v < 0 ? F : v);
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(slot, slots.data(), (size_t)T * 4, cudaMemcpyHostToDevice, run);
+    if (e == cudaSuccess) e = cudaMemsetAsync(frames, 0, (size_t)(F + 1) * N * ld * 4, run);
+  }
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample tables: %s", cudaGetErrorString(e));
   tc_prepare(h, run);
   const Plan& p = h->plan;
@@ -829,39 +921,30 @@ int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int3
     e = cudaMemcpyAsync(z, z_init, N * ld * 4, cudaMemcpyDeviceToDevice, run);
     if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "z_init copy: %s", cudaGetErrorString(e));
   } else {
-    launch_step_philox(run, p, h->d, 2, nullptr, nullptr, nullptr, nullptr, nullptr, seed, 0, nullptr, z);
+    launch_step_philox(run, p, h->d, 2, nullptr, nullptr, nullptr, nullptr, nullptr, seed, 0, nullptr, nullptr, z);
     h->launches++;
   }
 
-  // one reverse step, captured once and replayed T times; it reads the step, the seed and the first draw index from the
-  // device, and the coefficient table at a fixed address.  The key holds every device address the captured step bakes in
-  // (the chain buffers, the plan, the workspace, the weights and their tensor-core streams) next to the plan and weights
-  // epochs, so a buffer that moved for any reason forces a new capture instead of a replay through a freed pointer.
+  // one reverse step (and, with frames, the frame write), captured once and replayed T times; it reads the step, the seed
+  // and the first draw index from the device, and the coefficient table at a fixed address
   float* eps = static_cast<float*>(h->eps_buf.p);
   auto addr = [](const void* q) { return (long long)(uintptr_t)q; };
-  const std::vector<long long> key = {N, B, h->plan_epoch, h->weights_epoch, addr(h->smp_buf.p), addr(h->eps_buf.p),
-                                      addr(h->work_buf.p), addr(h->plan_buf.p), addr(h->rc_buf.p), addr(h->sched_buf.p),
-                                      addr(h->wbuf), addr(h->tc_blob.p), addr(h->tc_node_blob.p), addr(h->layers_dev.p)};
+  const std::vector<long long> key = chain_key(h, {N, B, F > 1, addr(h->smp_buf.p), addr(slot), addr(frames)});
   if (!h->smp_graph || key != h->smp_graph_key) {
-    if (h->smp_graph) cudaGraphExecDestroy(h->smp_graph);
-    h->smp_graph = nullptr;
     h->smp_graph_key.clear();
-    const int64_t before = h->launches;
-    cudaGraph_t g = nullptr;
-    e = cudaStreamBeginCapture(run, cudaStreamCaptureModeThreadLocal);
-    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample capture: %s", cudaGetErrorString(e));
-    int32_t rc = forward_impl(h, run, z, nullptr, coef, ctr, ctx, eps);
-    if (rc == BDIFF_OK) {
-      launch_step_philox(run, p, h->d, 0, z, eps, coef, ctr, ctr + 1, 0, 0, seed_draw, z);
+    rc = chain_capture(h, run, [&]() {
+      const int32_t r = forward_impl(h, run, z, nullptr, coef, ctr, ctx, eps);
+      if (r != BDIFF_OK) return r;
+      launch_step_philox(run, p, h->d, 0, z, eps, coef, ctr, F > 1 ? nullptr : ctr + 1, 0, 0, seed_draw, nullptr, z);
       h->launches++;
-    }
-    e = cudaStreamEndCapture(run, &g);
-    h->smp_step_launches = h->launches - before;
-    h->launches = before;
-    if (rc != BDIFF_OK) { if (g) cudaGraphDestroy(g); return rc; }
-    if (e == cudaSuccess) e = cudaGraphInstantiate(&h->smp_graph, g, 0);
-    if (g) cudaGraphDestroy(g);
-    if (e != cudaSuccess) { h->smp_graph = nullptr; return h->fail(BDIFF_ECUDA, "sample graph: %s", cudaGetErrorString(e)); }
+      if (F > 1) {
+        launch_write_frame(run, p, h->d, h->scfg.num_atom_types, h->scfg.norm_values, h->scfg.norm_biases, z, slot, ctr,
+                           ctr + 1, frames);
+        h->launches++;
+      }
+      return BDIFF_OK;
+    }, &h->smp_graph, &h->smp_step_launches);
+    if (rc != BDIFF_OK) return rc;
     h->smp_graph_key = key;
     h->smp_graph_builds++;
   }
@@ -870,20 +953,169 @@ int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int3
     h->launches += h->smp_step_launches;
   }
   if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample replay: %s", cudaGetErrorString(e));
+  return chain_tail(h, run, z, ctx, dec, seed, draw0 + 2ull * T, xhn, tot, frames, F, bi_dev, out, batch_index);
+}
 
-  // p(x, h | z_0) with draws draw0 + 2T, draw0 + 2T + 1, then the discretising tail of mol_gen_sample
-  int32_t rc = forward_impl(h, run, z, nullptr, dec, nullptr, ctx, eps);
-  if (rc != BDIFF_OK) return rc;
-  launch_step_philox(run, p, h->d, 1, z, eps, dec, nullptr, nullptr, seed, draw0 + 2ull * T, nullptr, xhn);
-  launch_sample_finish(run, p, h->d, h->scfg.num_atom_types, h->scfg.norm_values, h->scfg.norm_biases, xhn, xh, tot);
-  h->launches += 3;
-  if (batch_index) {
-    e = cudaMemcpyAsync(batch_index, bi_dev, N * 8, cudaMemcpyDeviceToDevice, run);
-    if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "batch_index copy: %s", cudaGetErrorString(e));
+int32_t bdiff_repaint_tables(const bdiff_sample_config* cfg, int32_t num_timesteps, int32_t num_resamplings,
+                             int32_t jump_length, int32_t return_frames, int32_t* num_ops, int32_t* num_jumps,
+                             float* rev_out, float* known_out, float* jump_out, float* decode_out, int32_t* op_s_out,
+                             int32_t* slot_out, uint8_t* jump_after_out, uint64_t* op_draw_out, uint64_t* jump_draw_out,
+                             uint64_t* decode_draw_out) {
+  if (!cfg || !num_ops || !num_jumps || sample_config_error(*cfg)) return BDIFF_EINVAL;
+  if (!repaint_args_error(num_timesteps, num_resamplings, jump_length, return_frames).empty()) return BDIFF_EINVAL;
+  const RepaintProgram g = repaint_program(schedule_gamma(cfg->model_timesteps, cfg->schedule_power, cfg->noise_precision),
+                                           num_resamplings, jump_length, num_timesteps, return_frames);
+  *num_ops = (int32_t)g.op_s.size();
+  *num_jumps = (int32_t)g.jump_draw.size();
+  if (rev_out) std::copy(g.rev.begin(), g.rev.end(), rev_out);
+  if (known_out) std::copy(g.known.begin(), g.known.end(), known_out);
+  if (jump_out) std::copy(g.jump.begin(), g.jump.end(), jump_out);
+  if (decode_out) std::copy(g.dec, g.dec + 4, decode_out);
+  if (op_s_out) std::copy(g.op_s.begin(), g.op_s.end(), op_s_out);
+  if (slot_out) std::copy(g.slot.begin(), g.slot.end(), slot_out);
+  if (jump_after_out) std::copy(g.jump_after.begin(), g.jump_after.end(), jump_after_out);
+  if (op_draw_out) std::copy(g.op_draw.begin(), g.op_draw.end(), op_draw_out);
+  if (jump_draw_out) std::copy(g.jump_draw.begin(), g.jump_draw.end(), jump_draw_out);
+  if (decode_draw_out) *decode_draw_out = g.decode_draw;
+  return BDIFF_OK;
+}
+
+int32_t bdiff_inpaint(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host, const float* context,
+                      int32_t num_timesteps, int32_t num_resamplings, int32_t jump_length, uint64_t seed,
+                      const float* xh0_host, const uint8_t* fixed_host, int32_t return_frames, const float* tables_host,
+                      float* out, int64_t* batch_index) {
+  if (!h) return BDIFF_EINVAL;
+  if (!h->have_sample_cfg) return h->fail(BDIFF_ESTATE, "bdiff_sample_setup has not been called");
+  const std::string why = inpaint_args_error(h->d.F, h->d.C, h->scfg, num_mols, num_nodes_host, context, num_timesteps,
+                                             num_resamplings, jump_length, return_frames, xh0_host, fixed_host, out);
+  if (!why.empty()) return h->fail(BDIFF_EINVAL, "bdiff_inpaint: %s", why.c_str());
+  if (bdiff_weights_missing(h) != 0) return h->fail(BDIFF_ESTATE, "%d parameters not set", bdiff_weights_missing(h));
+  const int B = num_mols, T = num_timesteps, F = return_frames, C = h->d.C, ld = 3 + h->d.F;
+  std::vector<int32_t> counts(num_nodes_host, num_nodes_host + B);
+  long long N = 0;
+  for (int32_t c : counts) N += c;
+  RepaintProgram g = repaint_program(schedule_gamma(h->scfg.model_timesteps, h->scfg.schedule_power,
+                                                    h->scfg.noise_precision),
+                                     num_resamplings, jump_length, T, F);
+  const size_t ops = g.op_s.size(), jumps = g.jump_draw.size();
+  if (tables_host) {      // the caller's rows, in bdiff_repaint_tables' order
+    const float* q = tables_host;
+    g.rev.assign(q, q + ops * 4);
+    q += ops * 4;
+    g.known.assign(q, q + ops * 2);
+    q += ops * 2;
+    g.jump.assign(q, q + jumps * 4);
+    q += jumps * 4;
+    std::copy(q, q + 4, g.dec);
   }
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "sample: %s", cudaGetErrorString(e));
-  return bdiff_check(h, run);
+  std::vector<float> xh0(xh0_host, xh0_host + N * ld);
+  center_on_fixed(B, num_nodes_host, ld, fixed_host, xh0.data());
+  cudaStream_t run;
+  int32_t rc = chain_stream(h, stream, &run);
+  if (rc != BDIFF_OK) return rc;
+
+  // per-atom buffers (their layout depends on the batch only) and the frames last; the program's tables each in a buffer
+  // of its own, so that a shorter program reuses every address the captured bodies read
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at += (bytes + 255) / 256 * 256; return o; };
+  const size_t o_bi = take(N * 8), o_mask = take(N), o_z = take(N * ld * 4), o_xhn = take(N * ld * 4),
+               o_ctx = take(N * C * 4), o_xh0 = take(N * ld * 4), o_fixed = take(N), o_ctr = take(48),
+               o_tot = take((size_t)B * 12), o_dec = take(16), o_frames = take(F > 1 ? (size_t)(F + 1) * N * ld * 4 : 0);
+  cudaError_t e = h->inp_buf.ensure(at);
+  if (e == cudaSuccess) e = h->inp_rev.ensure(ops * 16);
+  if (e == cudaSuccess) e = h->inp_known.ensure(ops * 8);
+  if (e == cudaSuccess) e = h->inp_slot.ensure(ops * 4);
+  if (e == cudaSuccess) e = h->inp_draw.ensure(ops * 8);
+  if (e == cudaSuccess) e = h->inp_jump.ensure(std::max<size_t>(jumps, 1) * 16);
+  if (e == cudaSuccess) e = h->inp_jdraw.ensure(std::max<size_t>(jumps, 1) * 8);
+  if (e != cudaSuccess) return h->fail(BDIFF_ENOMEM, "inpaint buffers: %s", cudaGetErrorString(e));
+  unsigned char* base = static_cast<unsigned char*>(h->inp_buf.p);
+  int64_t* bi_dev = reinterpret_cast<int64_t*>(base + o_bi);
+  float* z = reinterpret_cast<float*>(base + o_z);
+  float* xhn = reinterpret_cast<float*>(base + o_xhn);
+  float* ctx = C ? reinterpret_cast<float*>(base + o_ctx) : nullptr;
+  float* xh0_dev = reinterpret_cast<float*>(base + o_xh0);
+  uint8_t* fixed = base + o_fixed;
+  int* ctr = reinterpret_cast<int*>(base + o_ctr);                                   // {op, op done, jump, jump done}
+  // {seed, 0}: the known part's and the jump's draws are the table's; {seed, 2}: the unknown part's follow the known's
+  unsigned long long* seed_draw = reinterpret_cast<unsigned long long*>(base + o_ctr + 16);
+  float* tot = reinterpret_cast<float*>(base + o_tot);
+  float* dec = reinterpret_cast<float*>(base + o_dec);
+  float* frames = F > 1 ? reinterpret_cast<float*>(base + o_frames) : nullptr;
+  float* rev = static_cast<float*>(h->inp_rev.p);
+  float* known = static_cast<float*>(h->inp_known.p);
+  int* slot = static_cast<int*>(h->inp_slot.p);
+  unsigned long long* draw = static_cast<unsigned long long*>(h->inp_draw.p);
+  float* jump = static_cast<float*>(h->inp_jump.p);
+  unsigned long long* jdraw = static_cast<unsigned long long*>(h->inp_jdraw.p);
+
+  rc = chain_batch(h, run, counts, bi_dev, base + o_mask, &h->inp_counts, &h->inp_plan_epoch);
+  if (rc != BDIFF_OK) return rc;
+  const unsigned long long sd[4] = {seed, 0, seed, 2};
+  e = cudaMemcpyAsync(rev, g.rev.data(), ops * 16, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(known, g.known.data(), ops * 8, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(slot, g.slot.data(), ops * 4, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(draw, g.op_draw.data(), ops * 8, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess && jumps) e = cudaMemcpyAsync(jump, g.jump.data(), jumps * 16, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess && jumps) e = cudaMemcpyAsync(jdraw, g.jump_draw.data(), jumps * 8, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dec, g.dec, 16, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(xh0_dev, xh0.data(), N * ld * 4, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(fixed, fixed_host, N, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess) e = cudaMemsetAsync(ctr, 0, 16, run);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(seed_draw, sd, 32, cudaMemcpyHostToDevice, run);
+  if (e == cudaSuccess && frames) e = cudaMemsetAsync(frames, 0, (size_t)(F + 1) * N * ld * 4, run);
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "inpaint tables: %s", cudaGetErrorString(e));
+  tc_prepare(h, run);
+  const Plan& p = h->plan;
+  if (C) {
+    launch_gather_context(run, p, C, context, ctx);
+    h->launches++;
+  }
+  launch_step_philox(run, p, h->d, 2, nullptr, nullptr, nullptr, nullptr, nullptr, seed, 0, nullptr, nullptr, z);
+  h->launches++;
+
+  // the op body: reverse step to s, combination with the known part, frame write; it advances the op counter.  The jump
+  // body: the jump back at the jump counter, which it advances.
+  float* eps = static_cast<float*>(h->eps_buf.p);
+  auto addr = [](const void* q) { return (long long)(uintptr_t)q; };
+  const std::vector<long long> key = chain_key(h, {N, B, F > 1, addr(h->inp_buf.p), addr(rev), addr(known), addr(slot),
+                                                  addr(draw), addr(jump), addr(jdraw)});
+  if (!h->inp_op_graph || !h->inp_jump_graph || key != h->inp_graph_key) {
+    h->inp_graph_key.clear();
+    rc = chain_capture(h, run, [&]() {
+      const int32_t r = forward_impl(h, run, z, nullptr, rev, ctr, ctx, eps);
+      if (r != BDIFF_OK) return r;
+      launch_step_philox(run, p, h->d, 0, z, eps, rev, ctr, nullptr, 0, 0, seed_draw + 2, draw, z);
+      launch_repaint_combine_philox(run, p, h->d, z, xh0_dev, fixed, known, ctr, frames ? nullptr : ctr + 1, seed_draw,
+                                    draw);
+      h->launches += 2;
+      if (frames) {
+        launch_write_frame(run, p, h->d, h->scfg.num_atom_types, h->scfg.norm_values, h->scfg.norm_biases, z, slot, ctr,
+                           ctr + 1, frames);
+        h->launches++;
+      }
+      return BDIFF_OK;
+    }, &h->inp_op_graph, &h->inp_op_launches);
+    if (rc == BDIFF_OK)
+      rc = chain_capture(h, run, [&]() {
+        launch_step_philox(run, p, h->d, 3, z, nullptr, jump, ctr + 2, ctr + 3, 0, 0, seed_draw, jdraw, z);
+        h->launches++;
+        return BDIFF_OK;
+      }, &h->inp_jump_graph, &h->inp_jump_launches);
+    if (rc != BDIFF_OK) return rc;
+    h->inp_graph_key = key;
+    h->inp_graph_builds++;
+  }
+  for (size_t i = 0; i < ops && e == cudaSuccess; ++i) {
+    e = cudaGraphLaunch(h->inp_op_graph, run);
+    h->launches += h->inp_op_launches;
+    if (e == cudaSuccess && g.jump_after[i]) {
+      e = cudaGraphLaunch(h->inp_jump_graph, run);
+      h->launches += h->inp_jump_launches;
+    }
+  }
+  if (e != cudaSuccess) return h->fail(BDIFF_ECUDA, "inpaint replay: %s", cudaGetErrorString(e));
+  return chain_tail(h, run, z, ctx, dec, seed, g.decode_draw, xhn, tot, frames, F, bi_dev, out, batch_index);
 }
 
 }  // extern "C"

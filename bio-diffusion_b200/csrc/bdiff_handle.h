@@ -104,6 +104,14 @@ struct bdiff_handle {
   std::vector<long long> smp_graph_key;
   int64_t smp_step_launches = 0;        // kernels in one captured reverse step
   int64_t smp_graph_builds = 0;
+  DevBuf smp_slot, smp_frames;          // bdiff_sample_frames: frame slot per step, frame rows (+ the dummy slot)
+  // bdiff_inpaint: the chain's per-atom buffers, the program's tables, and the captured op and jump bodies
+  DevBuf inp_buf, inp_rev, inp_known, inp_slot, inp_draw, inp_jump, inp_jdraw;
+  std::vector<int32_t> inp_counts;
+  int inp_plan_epoch = -1;
+  cudaGraphExec_t inp_op_graph = nullptr, inp_jump_graph = nullptr;
+  std::vector<long long> inp_graph_key;
+  int64_t inp_op_launches = 0, inp_jump_launches = 0, inp_graph_builds = 0;
 
   int fail(int code, const char* fmt, ...) {
     char buf[512];

@@ -52,16 +52,22 @@ void launch_step(cudaStream_t st, const Plan& p, const Dims& d, int mode, const 
 void launch_repaint_combine(cudaStream_t st, const Plan& p, const Dims& d, float* z, const float* xh0,
                             const uint8_t* fixed, const float* noise_x, const float* noise_h,
                             const float* known_table, const int* op_ptr);
-// the native chain of bdiff_sample: step kernels with in-kernel Philox noise (bdiff_philox.cuh), the noise itself, the
+// the native chains of bdiff_sample / bdiff_inpaint: step and RePaint kernels with in-kernel Philox noise (bdiff_philox.cuh), the noise itself, the
 // per-atom context and the discretising tail
 void launch_step_philox(cudaStream_t st, const Plan& p, const Dims& d, int mode, const float* z, const float* eps,
                         const float* coef_table, int* step_ptr, int* done, unsigned long long seed,
-                        unsigned long long draw0, const unsigned long long* seed_draw, float* out);
+                        unsigned long long draw0, const unsigned long long* seed_draw,
+                        const unsigned long long* draw_table, float* out);
+void launch_repaint_combine_philox(cudaStream_t st, const Plan& p, const Dims& d, float* z, const float* xh0,
+                                   const uint8_t* fixed, const float* known_table, int* op_ptr, int* done,
+                                   const unsigned long long* seed_draw, const unsigned long long* draw_table);
+void launch_write_frame(cudaStream_t st, const Plan& p, const Dims& d, int A, const float* nv, const float* nb,
+                        const float* z, const int* slot, int* step_ptr, int* done, float* frames);
 void launch_noise_fill(cudaStream_t st, unsigned long long seed, unsigned long long draw, long long n, float* out);
 void launch_philox_fill(cudaStream_t st, unsigned long long seed, unsigned long long draw, long long blocks, uint32_t* out);
 void launch_gather_context(cudaStream_t st, const Plan& p, int C, const float* context, float* ctx);
 void launch_sample_finish(cudaStream_t st, const Plan& p, const Dims& d, int A, const float* nv, const float* nb,
-                          const float* xhn, float* out, float* tot);
+                          const float* xhn, float* out, float* tot, bool cog_fix);
 void launch_edge_index(cudaStream_t st, const Plan& p, long long* out);
 void launch_edge_rc(cudaStream_t st, const Plan& p, int4* out, long long n);
 // one slice of a reference parameter tensor -> kernel layout (see k_pack_multi)

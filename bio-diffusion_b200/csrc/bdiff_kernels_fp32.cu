@@ -926,13 +926,28 @@ __global__ void __launch_bounds__(128) k_repaint_combine(Plan p, Dims d, float* 
 }
 
 // ------------------------------------------------------------------------------- native chain (bdiff_sample)
+// The last CTA of a grid to get here (every CTA has read *ctr by then) stores value into *ctr and re-arms *done, so a
+// counter a kernel reads is advanced without another launch.
+__device__ __forceinline__ void advance_counter(int* ctr, int* done, int value) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(done, 1) == (int)gridDim.x - 1) {
+      *done = 0;
+      *ctr = value;
+    }
+  }
+}
+
 // k_step with the noise computed in place: noise_x = draw dx, noise_h = draw dx + 1 of `seed` (bdiff_philox.cuh), where
-// dx = draw0 + 2 * *step_ptr in mode 0 and draw0 otherwise ({seed, draw0} = seed_draw[0..1] when seed_draw is given).  Masking, centring and every arithmetic step are k_step's.
-// Mode 0 also advances the step counter: the last CTA to finish (all CTAs have read it by then) adds 1 and re-arms `done`.
+// dx = draw0 + draw_table[*step_ptr] when a draw table is given (RePaint programs), else draw0 + 2 * *step_ptr in mode 0
+// and draw0 otherwise ({seed, draw0} = seed_draw[0..1] when seed_draw is given).  Masking, centring and every arithmetic
+// step are k_step's, mode 3 included.  Modes 0 and 3 advance the step counter when `done` is given.
 __global__ void __launch_bounds__(128) k_step_philox(Plan p, Dims d, int mode, const float* __restrict__ z,
                                                      const float* __restrict__ eps, const float* __restrict__ coef_table,
                                                      int* step_ptr, int* done, unsigned long long seed,
                                                      unsigned long long draw0, const unsigned long long* seed_draw,
+                                                     const unsigned long long* __restrict__ draw_table,
                                                      float* __restrict__ out) {
   const int step = step_ptr ? *step_ptr : 0;
   if (seed_draw) {            // a captured step reads {seed, draw0} from the device, so one graph serves every seed
@@ -940,7 +955,8 @@ __global__ void __launch_bounds__(128) k_step_philox(Plan p, Dims d, int mode, c
     draw0 = seed_draw[1];
   }
   const float* coef = coef_table ? coef_table + 4 * step : nullptr;
-  const unsigned long long dx = draw0 + (mode == 0 ? 2ull * (unsigned)step : 0ull), dh = dx + 1;
+  const unsigned long long dx = draw0 + (draw_table ? draw_table[step] : mode == 0 ? 2ull * (unsigned)step : 0ull),
+                           dh = dx + 1;
   __shared__ float red[4][4];
   const int k = blockIdx.x;
   const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
@@ -970,12 +986,13 @@ __global__ void __launch_bounds__(128) k_step_philox(Plan p, Dims d, int mode, c
       float v;
       if (mode == 0) v = z[(size_t)i * ld + c] / c0 - c1 * eps[(size_t)i * ld + c] + c2 * nz;
       else if (mode == 1) v = c0 * (z[(size_t)i * ld + c] - c1 * eps[(size_t)i * ld + c]) + c2 * nz;
+      else if (mode == 3) v = c0 * z[(size_t)i * ld + c] + c1 * nz;
       else v = nz;
       out[(size_t)i * ld + c] = v;
       if (c < 3) t[c] += v;
     }
   }
-  if (mode != 0) return;
+  if (mode == 1 || mode == 2) return;
   block_sum4(t, red);
   const float zx = cnt > 0.f ? t[0] / cnt : 0.f, zy = cnt > 0.f ? t[1] / cnt : 0.f, zz = cnt > 0.f ? t[2] / cnt : 0.f;
   for (int i = n0 + threadIdx.x; i < n1; i += 128) {
@@ -984,15 +1001,87 @@ __global__ void __launch_bounds__(128) k_step_philox(Plan p, Dims d, int mode, c
     out[(size_t)i * ld + 1] -= zy * m;
     out[(size_t)i * ld + 2] -= zz * m;
   }
-  if (!step_ptr) return;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(done, 1) == (int)gridDim.x - 1) {
-      *done = 0;
-      *step_ptr = step + 1;
+  if (done) advance_counter(step_ptr, done, step + 1);
+}
+
+// k_repaint_combine with the known part's noise computed in place: noise_x = draw dk, noise_h = draw dk + 1 of the seed,
+// dk = seed_draw[1] + draw_table[*op_ptr], element layouts as in k_step_philox.  Advances the op counter when `done` is
+// given.
+__global__ void __launch_bounds__(128) k_repaint_combine_philox(Plan p, Dims d, float* __restrict__ z,
+                                                                const float* __restrict__ xh0,
+                                                                const uint8_t* __restrict__ fixed,
+                                                                const float* __restrict__ known_table, int* op_ptr,
+                                                                int* done, const unsigned long long* seed_draw,
+                                                                const unsigned long long* __restrict__ draw_table) {
+  __shared__ float red[4][4];
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const int ld = 3 + d.F;
+  const int op = *op_ptr;
+  const unsigned long long seed = seed_draw[0], dk = seed_draw[1] + draw_table[op], dkh = dk + 1;
+  const float alpha = __ldg(known_table + 2 * op), sigma = __ldg(known_table + 2 * op + 1);
+  float s[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float m = p.mask[i] ? 1.f : 0.f;
+    s[0] += philox_normal(seed, dk, (unsigned long long)i * 3 + 0) * m;
+    s[1] += philox_normal(seed, dk, (unsigned long long)i * 3 + 1) * m;
+    s[2] += philox_normal(seed, dk, (unsigned long long)i * 3 + 2) * m;
+    s[3] += m;
+  }
+  block_sum4(s, red);
+  const float cnt = s[3];
+  const float nc[3] = {cnt > 0.f ? s[0] / cnt : 0.f, cnt > 0.f ? s[1] / cnt : 0.f, cnt > 0.f ? s[2] / cnt : 0.f};
+  float u[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    if (!fixed[i]) continue;
+    const float m = p.mask[i] ? 1.f : 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      u[c] += z[(size_t)i * ld + c];
+      q[c] += alpha * xh0[(size_t)i * ld + c] + sigma * ((philox_normal(seed, dk, (unsigned long long)i * 3 + c) - nc[c] * m) * m);
+    }
+    u[3] += 1.f;
+  }
+  block_sum4(u, red);
+  block_sum4(q, red);
+  const float nf = u[3];
+  if (nf != 0.f) {                                       // no fixed atom: the molecule is sampled freely
+    const float sh[3] = {u[0] / nf - q[0] / nf, u[1] / nf - q[1] / nf, u[2] / nf - q[2] / nf};
+    for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+      if (!fixed[i]) continue;
+      const float m = p.mask[i] ? 1.f : 0.f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        z[(size_t)i * ld + c] =
+            (alpha * xh0[(size_t)i * ld + c] + sigma * ((philox_normal(seed, dk, (unsigned long long)i * 3 + c) - nc[c] * m) * m)) + sh[c];
+      for (int f = 0; f < d.F; ++f)
+        z[(size_t)i * ld + 3 + f] =
+            alpha * xh0[(size_t)i * ld + 3 + f] + sigma * (philox_normal(seed, dkh, (unsigned long long)i * d.F + f) * m);
     }
   }
+  if (done) advance_counter(op_ptr, done, op + 1);
+}
+
+// frames[slot[*step_ptr]] = unnormalize_z(z) (sampler.py _write_frame; every atom present, so the mask factor is 1), with
+// torch's rounding: each multiply and add rounded on its own.  Then advances the step counter.
+__global__ void __launch_bounds__(128) k_write_frame(Plan p, Dims d, int A, float nv0, float nv1, float nb1, float nv2,
+                                                     float nb2, const float* __restrict__ z,
+                                                     const int* __restrict__ slot, int* step_ptr, int* done,
+                                                     float* __restrict__ frames) {
+  const int step = *step_ptr;
+  const int k = blockIdx.x;
+  const int n0 = p.mol_off[k], n1 = p.mol_off[k + 1];
+  const int ld = 3 + d.F;
+  float* fr = frames + (size_t)slot[step] * p.N * ld;
+  for (int i = n0 + threadIdx.x; i < n1; i += 128) {
+    const float* row = z + (size_t)i * ld;
+    float* o = fr + (size_t)i * ld;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = __fmul_rn(row[c], nv0);
+    for (int a = 0; a < A; ++a) o[3 + a] = __fadd_rn(__fmul_rn(row[3 + a], nv1), nb1);
+    if (ld > 3 + A) o[3 + A] = __fadd_rn(__fmul_rn(row[3 + A], nv2), nb2);
+  }
+  advance_counter(step_ptr, done, step + 1);
 }
 
 __global__ void k_noise_fill(unsigned long long seed, unsigned long long draw, long long n, float* __restrict__ out) {
@@ -1168,8 +1257,19 @@ void launch_repaint_combine(cudaStream_t st, const Plan& p, const Dims& d, float
 }
 void launch_step_philox(cudaStream_t st, const Plan& p, const Dims& d, int mode, const float* z, const float* eps,
                         const float* coef_table, int* step_ptr, int* done, unsigned long long seed,
-                        unsigned long long draw0, const unsigned long long* seed_draw, float* out) {
-  k_step_philox<<<p.B, 128, 0, st>>>(p, d, mode, z, eps, coef_table, step_ptr, done, seed, draw0, seed_draw, out);
+                        unsigned long long draw0, const unsigned long long* seed_draw,
+                        const unsigned long long* draw_table, float* out) {
+  k_step_philox<<<p.B, 128, 0, st>>>(p, d, mode, z, eps, coef_table, step_ptr, done, seed, draw0, seed_draw, draw_table,
+                                     out);
+}
+void launch_repaint_combine_philox(cudaStream_t st, const Plan& p, const Dims& d, float* z, const float* xh0,
+                                   const uint8_t* fixed, const float* known_table, int* op_ptr, int* done,
+                                   const unsigned long long* seed_draw, const unsigned long long* draw_table) {
+  k_repaint_combine_philox<<<p.B, 128, 0, st>>>(p, d, z, xh0, fixed, known_table, op_ptr, done, seed_draw, draw_table);
+}
+void launch_write_frame(cudaStream_t st, const Plan& p, const Dims& d, int A, const float* nv, const float* nb,
+                        const float* z, const int* slot, int* step_ptr, int* done, float* frames) {
+  k_write_frame<<<p.B, 128, 0, st>>>(p, d, A, nv[0], nv[1], nb[1], nv[2], nb[2], z, slot, step_ptr, done, frames);
 }
 void launch_noise_fill(cudaStream_t st, unsigned long long seed, unsigned long long draw, long long n, float* out) {
   if (n > 0) k_noise_fill<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(seed, draw, n, out);
@@ -1182,9 +1282,9 @@ void launch_gather_context(cudaStream_t st, const Plan& p, int C, const float* c
   if (n > 0) k_gather_context<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(p, C, context, ctx);
 }
 void launch_sample_finish(cudaStream_t st, const Plan& p, const Dims& d, int A, const float* nv, const float* nb,
-                          const float* xhn, float* out, float* tot) {
+                          const float* xhn, float* out, float* tot, bool cog_fix) {
   k_sample_finish<<<p.B, 128, 0, st>>>(p, d, A, nv[0], nv[1], nb[1], nv[2], nb[2], xhn, out, tot);
-  k_sample_cog_fix<<<p.B, 128, 0, st>>>(p, d, tot, out);
+  if (cog_fix) k_sample_cog_fix<<<p.B, 128, 0, st>>>(p, d, tot, out);
 }
 void launch_edge_index(cudaStream_t st, const Plan& p, long long* out) {
   if (p.E > 0) k_edge_index<<<(unsigned)((p.E + 255) / 256), 256, 0, st>>>(p, out);

@@ -1,4 +1,5 @@
-// bdiff_schedule.h — the host half of bdiff_sample: the noise schedule's tables and the argument checks.  Plain C++17
+// bdiff_schedule.h — the host half of bdiff_sample and bdiff_inpaint: the noise schedule's tables, the RePaint program,
+// the centring of the inpainted molecules and the argument checks.  Plain C++17
 // without CUDA headers, so that the CPU suite compiles it with g++ (tests/native/sample_hostcheck.cpp).
 //
 // The tables restate bdiff/schedule.py (gamma_table, step_coefficient_table, decode_coefficients).  gamma is fp64 exactly
@@ -112,6 +113,156 @@ inline std::string sample_args_error(int num_h, int num_context, const bdiff_sam
     }
   }
   if (!xh) return "xh is NULL";
+  return "";
+}
+
+// The RePaint program of inpaint, unrolled (bdiff/schedule.py repaint_schedule / repaint_program).  Every denoise op moves
+// z from t = s+1 to s; the last op of every segment but the final one is followed by a jump back from s to t = s + j.
+// Draws (include/bdiff.h): z_T takes 0 and 1; then in chain order each op takes 4 (known x, known h, unknown x, unknown h)
+// and each jump 2 (x, h); the decode takes the last 2.
+struct RepaintProgram {
+  std::vector<int32_t> sched;          // denoising ops of each segment (get_repaint_schedule)
+  std::vector<int32_t> op_s;           // [ops] grid point s each op lands on
+  std::vector<uint8_t> jump_after;     // [ops] 1: a jump back follows the op
+  std::vector<int32_t> slot;           // [ops] frame slot of the op; return_frames = the dummy slot (no frame)
+  std::vector<float> rev;              // [ops * 4] {alpha_ts, c_eps, sigma, t}: rows of schedule_tables
+  std::vector<float> known;            // [ops * 2] {alpha_s, sigma_s}
+  std::vector<float> jump;             // [jumps * 4] {alpha_t|s, sigma_t|s, s, t}
+  std::vector<uint64_t> op_draw;       // [ops] the op's first draw (known x)
+  std::vector<uint64_t> jump_draw;     // [jumps] the jump's first draw (x)
+  uint64_t decode_draw = 0;            // the decode's first draw
+  float dec[4] = {0.f, 0.f, 0.f, 0.f}; // the decode row of schedule_tables
+};
+
+// Why a chain of num_timesteps steps cannot return `return_frames` frames ("" = it can): schedule.py check_frames.
+inline std::string frames_args_error(int num_timesteps, int return_frames) {
+  char buf[160];
+  if (!(0 < return_frames && return_frames <= num_timesteps)) {
+    snprintf(buf, sizeof buf, "return_frames must be in [1, num_timesteps=%d], got %d", num_timesteps, return_frames);
+    return buf;
+  }
+  if (num_timesteps % return_frames) {
+    snprintf(buf, sizeof buf, "return_frames=%d does not divide num_timesteps=%d", return_frames, num_timesteps);
+    return buf;
+  }
+  return "";
+}
+
+// Why a RePaint program cannot be built ("" = it can): check_repaint of schedule.py.
+inline std::string repaint_args_error(int num_timesteps, int resamplings, int jump_length, int return_frames) {
+  if (resamplings < 1 || jump_length < 1 || num_timesteps < 1) {
+    char buf[160];
+    snprintf(buf, sizeof buf, "num_resamplings, jump_length and num_timesteps must be >= 1 (got %d, %d, %d)", resamplings,
+             jump_length, num_timesteps);
+    return buf;
+  }
+  const std::string why = frames_args_error(num_timesteps, return_frames);
+  if (!why.empty()) return why;
+  if (jump_length > 1 && return_frames > 1) return "chain visualisation (return_frames > 1) is only defined for jump_length == 1";
+  return "";
+}
+
+// Frame slot written after the step that lands on s (schedule.py frame_slot), or -1.
+inline int frame_slot(long long s, long long num_timesteps, long long return_frames) {
+  return (s * return_frames) % num_timesteps == 0 ? (int)(s * return_frames / num_timesteps) : -1;
+}
+
+// The program for arguments repaint_args_error accepts.  Reverse rows are gathered from schedule_tables(gamma, T), so an
+// op is bit-identical to bdiff_sample's step at the same s; the known and jump rows are evaluated in fp64 at the fp32 grid
+// and gamma values like schedule_tables' and rounded once.
+inline RepaintProgram repaint_program(const std::vector<float>& gamma, int resamplings, int jump_length, int num_timesteps,
+                                      int return_frames) {
+  RepaintProgram g;
+  const int T = num_timesteps, J = jump_length, TM = (int)gamma.size() - 1;
+  for (int curr = 0; curr < T;) {                        // get_repaint_schedule, built back to front
+    if (curr + J < T) {
+      if (!g.sched.empty()) g.sched.back() += J;
+      g.sched.insert(g.sched.end(), g.sched.empty() ? resamplings : resamplings - 1, J);
+      curr += J;
+    } else {
+      if (!g.sched.empty()) g.sched.back() += T - curr;
+      else g.sched.push_back(T - curr);
+      curr = T;
+    }
+  }
+  std::vector<int32_t> sched(g.sched.rbegin(), g.sched.rend());
+  g.sched = sched;
+  std::vector<float> coef((size_t)T * 4);
+  schedule_tables(gamma, T, coef.data(), g.dec);
+  auto gam = [&](float v) { return (double)gamma[(size_t)nearbyintf(v * (float)TM)]; };
+  uint64_t draw = 2;
+  int s = T - 1;
+  for (size_t i = 0; i < sched.size(); ++i) {
+    const bool last_seg = i + 1 == sched.size();
+    for (int jj = 0; jj < sched[i]; ++jj) {
+      g.op_s.push_back(s);
+      const int slot = sched[i] > J || last_seg ? frame_slot(s, T, return_frames) : -1;
+      g.slot.push_back(slot < 0 ? return_frames : slot);
+      g.rev.insert(g.rev.end(), coef.begin() + 4 * (size_t)(T - 1 - s), coef.begin() + 4 * (size_t)(T - s));
+      const double g_s = gam((float)s / (float)T);
+      g.known.push_back((float)std::sqrt(d_sigmoid(-g_s)));
+      g.known.push_back((float)std::sqrt(d_sigmoid(g_s)));
+      g.op_draw.push_back(draw);
+      draw += 4;
+      const bool jump = jj == sched[i] - 1 && !last_seg;
+      g.jump_after.push_back(jump ? 1 : 0);
+      if (jump) {
+        const float js = (float)s / (float)T, jt = (float)(s + J) / (float)T;
+        const double a_s = gam(js), a_t = gam(jt);
+        const double sigma2_ts = -std::expm1(d_softplus(a_s) - d_softplus(a_t));
+        g.jump.push_back((float)std::exp(0.5 * (d_logsigmoid(-a_t) - d_logsigmoid(-a_s))));
+        g.jump.push_back((float)std::sqrt(sigma2_ts));
+        g.jump.push_back(js);
+        g.jump.push_back(jt);
+        g.jump_draw.push_back(draw);
+        draw += 2;
+        s += J;
+      }
+      --s;
+    }
+  }
+  g.decode_draw = draw;
+  return g;
+}
+
+// xh0[:, :3] -= the mean position of the molecule's fixed atoms (GCDMSampler.inpaint): sequential fp32 sums of x * fixed
+// over the molecule's atoms in order, the count of fixed atoms, and the mean tot / max(count, 1), so a molecule without
+// fixed atoms is not moved.  xh0 is [N, ld] row-major.
+inline void center_on_fixed(int num_mols, const int32_t* num_nodes, int ld, const uint8_t* fixed, float* xh0) {
+  for (int k = 0, i0 = 0; k < num_mols; i0 += num_nodes[k++]) {
+    float tot[3] = {0.f, 0.f, 0.f}, cnt = 0.f;
+    for (int i = i0; i < i0 + num_nodes[k]; ++i) {
+      const float f = fixed[i] ? 1.f : 0.f;
+      for (int c = 0; c < 3; ++c) tot[c] += xh0[(size_t)i * ld + c] * f;
+      cnt += f;
+    }
+    const float div = std::fmax(cnt, 1.f);
+    const float mean[3] = {tot[0] / div, tot[1] / div, tot[2] / div};
+    for (int i = i0; i < i0 + num_nodes[k]; ++i)
+      for (int c = 0; c < 3; ++c) xh0[(size_t)i * ld + c] -= mean[c];
+  }
+}
+
+// Why bdiff_inpaint refuses its arguments ("" = accepted).
+inline std::string inpaint_args_error(int num_h, int num_context, const bdiff_sample_config& c, int num_mols,
+                                      const int32_t* num_nodes_host, const float* context, int num_timesteps,
+                                      int resamplings, int jump_length, int return_frames, const float* xh0_host,
+                                      const uint8_t* fixed_host, const float* out) {
+  std::string why = sample_args_error(num_h, num_context, c, num_mols, num_nodes_host, context, num_timesteps, nullptr,
+                                      nullptr, out);
+  if (!why.empty()) return why;
+  why = repaint_args_error(num_timesteps, resamplings, jump_length, return_frames);
+  if (!why.empty()) return why;
+  if (!xh0_host) return "xh0_host is NULL";
+  if (!fixed_host) return "fixed_host is NULL";
+  long long n = 0;
+  for (int k = 0; k < num_mols; ++k) n += num_nodes_host[k];
+  for (long long i = 0; i < n; ++i)
+    if (fixed_host[i] > 1) {
+      char buf[96];
+      snprintf(buf, sizeof buf, "fixed_host[%lld] = %d: must be 0 or 1", i, (int)fixed_host[i]);
+      return buf;
+    }
   return "";
 }
 

@@ -231,8 +231,61 @@ BDIFF_API int32_t bdiff_philox_fill(void* stream, uint64_t seed, uint64_t draw_i
 BDIFF_API int32_t bdiff_sample(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host,
                                const float* context, int32_t num_timesteps, uint64_t seed, const float* z_init,
                                const int64_t* z_init_shape, const float* tables_host, float* xh, int64_t* batch_index);
+/* bdiff_sample returning the chain's frames (mol_gen_sample's return_frames, :1309-1310, 1353-1360, 1404-1410):
+ * return_frames = F divides num_timesteps; out fp32[F, N, 3+num_h] (device): out[0] = the molecules, without the CoG drift
+ * fix (as the reference), out[k] = the unnormalised latent [x * nv0 | h * nv + nb] after the step that lands on
+ * s = k * num_timesteps / F.  Same draws as bdiff_sample; bdiff_sample is the case F = 1. */
+BDIFF_API int32_t bdiff_sample_frames(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host,
+                                      const float* context, int32_t num_timesteps, uint64_t seed, const float* z_init,
+                                      const int64_t* z_init_shape, int32_t return_frames, const float* tables_host,
+                                      float* out, int64_t* batch_index);
 /* Number of reverse-step graphs bdiff_sample has captured on this handle (cache diagnostics). */
 BDIFF_API int64_t bdiff_sample_graph_builds(const bdiff_handle* h);
+
+/* ---- inpainting through the C ABI alone -------------------------------------------------------------------------------
+ * Replaces: EquivariantVariationalDiffusion.inpaint (variational_diffusion.py:1580-1789, RePaint) as one call, with the two
+ * repairs of bdiff_renoise / GCDMSampler.inpaint (the dead self-conditioning line is dropped; the jump back takes
+ * alpha_t|s per molecule).  Sequence: as for bdiff_sample (bdiff_sample_setup first), then bdiff_inpaint.
+ *
+ * The RePaint program: get_repaint_schedule (:1549-1578) unrolled into denoise ops (a reverse step to s followed by the
+ * combination with the known part) and jumps back from s to s + jump_length.  Draws, in chain order: z_T takes 0 (x) and
+ * 1 (h); each op takes 4 (known x, known h, unknown x, unknown h); each jump takes 2 (x, h); the decode takes the last 2.
+ * Element layouts and values are those of bdiff_sample's draws, so GCDMSampler.inpaint(noise=philox_noise(seed)) replays
+ * the chain.
+ *
+ * bdiff_repaint_tables (host only): the program for (num_timesteps, num_resamplings, jump_length, return_frames), with
+ * the coefficients of bdiff_schedule_tables' precision contract.  *num_ops and *num_jumps are always written; every other
+ * output is written when non-NULL, so a call with NULL outputs is the size query:
+ *   rev_out   [ops * 4]   {alpha_ts, c_eps, sigma, t} of the op's reverse step (rows of bdiff_schedule_tables)
+ *   known_out [ops * 2]   {alpha_s, sigma_s}: z_known = alpha_s * xh0 + sigma_s * noise
+ *   jump_out  [jumps * 4] {alpha_t|s, sigma_t|s, s, t}
+ *   decode_out[4]         bdiff_schedule_tables' decode row
+ *   op_s_out [ops] grid point of the op, slot_out [ops] frame slot (return_frames = no frame), jump_after_out [ops] 0/1,
+ *   op_draw_out [ops] / jump_draw_out [jumps] first draw of the op / jump, *decode_draw_out first draw of the decode. */
+BDIFF_API int32_t bdiff_repaint_tables(const bdiff_sample_config* cfg, int32_t num_timesteps, int32_t num_resamplings,
+                                       int32_t jump_length, int32_t return_frames, int32_t* num_ops, int32_t* num_jumps,
+                                       float* rev_out, float* known_out, float* jump_out, float* decode_out,
+                                       int32_t* op_s_out, int32_t* slot_out, uint8_t* jump_after_out,
+                                       uint64_t* op_draw_out, uint64_t* jump_draw_out, uint64_t* decode_draw_out);
+
+/* The whole inpainting chain: xh0's positions centred on the fixed atoms of each molecule (sequential fp32 sums; a
+ * molecule without fixed atoms is not moved), z_T, the RePaint program from two captured CUDA graphs (op and jump, cached
+ * on the handle like bdiff_sample's), the decode and bdiff_sample's tail (the CoG drift fix only when return_frames = 1).
+ * Ends with bdiff_check (synchronises `stream`).
+ *   num_nodes_host, context, batch_index  as in bdiff_sample
+ *   xh0_host     fp32[N, 3+num_h] (host) the molecules [x | one_hot | charges], unnormalised as the reference passes them
+ *   fixed_host   uint8[N] (host) 1 = the atom keeps its type and position
+ *   num_resamplings >= 1, jump_length >= 1; return_frames = F divides num_timesteps and F > 1 needs jump_length = 1
+ *   tables_host  NULL (the library's program) or, for a program of O ops and J jumps (bdiff_repaint_tables), O*4 reverse
+ *                rows, O*2 known rows, J*4 jump rows and the decode row (host floats) to run on tables computed elsewhere
+ *   out          fp32[N, 3+num_h], or [F, N, 3+num_h] with out[0] = the molecules, out[k] = the latent after the op that
+ *                lands on s = k * num_timesteps / F (device) */
+BDIFF_API int32_t bdiff_inpaint(bdiff_handle* h, void* stream, int32_t num_mols, const int32_t* num_nodes_host,
+                                const float* context, int32_t num_timesteps, int32_t num_resamplings, int32_t jump_length,
+                                uint64_t seed, const float* xh0_host, const uint8_t* fixed_host, int32_t return_frames,
+                                const float* tables_host, float* out, int64_t* batch_index);
+/* Number of (op, jump) graph pairs bdiff_inpaint has captured on this handle (cache diagnostics). */
+BDIFF_API int64_t bdiff_inpaint_graph_builds(const bdiff_handle* h);
 
 /* ---- optimiser side of a training step (SURVEY.md §8 a21): adaptive gradient-norm clipping + AdamW(amsgrad) + EMA --
  * Replaces, per step: get_grad_norm + Queue statistics + clip_gradients (qm9_mol_gen_ddpm.py:1267-1304,

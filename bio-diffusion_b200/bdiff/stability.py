@@ -96,10 +96,8 @@ def bond_orders_batch(positions: torch.Tensor, atom_types: torch.Tensor, num_nod
             for k in ("bonds1", "bonds2", "bonds3")]
     x = positions.detach().to(torch.float32).contiguous()
     t = atom_types.detach().to(torch.int32).contiguous()
-    nn = num_nodes.detach().to(torch.int64).cpu()
+    nn = _check_batch(x, t, num_nodes, a)                     # a type outside the decoder would index past the tables
     n = int(x.shape[0])
-    if x.shape != (n, 3) or t.shape != (n,) or int(nn.sum()) != n or (nn < 0).any():
-        raise ValueError("positions [N,3], atom_types [N] and num_nodes (summing to N) expected")
     b = int(nn.numel())
     off = torch.zeros(b + 1, dtype=torch.int32)
     off[1:] = torch.cumsum(nn, 0).to(torch.int32)
